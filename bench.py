@@ -25,6 +25,8 @@ import numpy as np
 
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
+sys.dont_write_bytecode = True  # the tree may be read-only: no __pycache__ next to the sources
+os.environ["PYTHONDONTWRITEBYTECODE"] = "1"  # (nor from the side-measurement child processes)
 
 METRIC = "curl-curl+mass operator apply throughput"
 UNIT = "MDoF/s"
@@ -46,7 +48,15 @@ def parse():
     ap.add_argument("--cpu-sample-elems", type=int, default=0, help="elements in the CPU baseline sample (0 = auto)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-experiments", action="store_true", help="skip the opt-in kernel variants measured in subprocesses")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the last step's result y = A x (float64) to DIR/y.npy (rank r > 0: DIR/y_rank<r>.npy); "
+                         "x and the mesh are fixed by the arguments, so runs of two builds compare output for output")
     return ap.parse_args()
+
+
+def dump_outputs(directory, rank, y):
+    os.makedirs(directory, exist_ok=True)
+    np.save(os.path.join(directory, "y.npy" if rank == 0 else f"y_rank{rank}.npy"), np.ascontiguousarray(y, dtype=np.float64))
 
 
 def build_problem(n, p, warp, mesh_order=1, origin=(0.0, 0.0, 0.0), size=(1.0, 1.0, 1.0), coefficient="iso"):
@@ -124,7 +134,7 @@ def measured_peak_gbs():
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+        return 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3), not measured"
 
 
 def cpu_quota():
@@ -218,6 +228,8 @@ def run_reference(args, rank, world):
                          "min_ms": 1e3 * dts[0], "max_ms": 1e3 * dts[-1]},
         "e2e": {"value": value, "unit": UNIT, "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0},
     }
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, 0, ref.y)  # the last timed step's y (the arm zero-fills y before every step)
     print(json.dumps(line), flush=True)
 
 
@@ -243,7 +255,6 @@ def run_experiments(args):
     headline numbers) and printed as ITS OWN short JSON line -- {"experiment": name, ...} -- before the headline line, so that
     none of them can fall off a log tail. The headline line stays the last line of the output."""
     # no experiment STARTS after budget_s; each is cut off at 150 s, so the side measurements end within ~7 minutes in the worst case
-    # (they took 1.5 minutes on B200 with the round-2 list of 13, profiles/r02_bench_n1_with_experiments.jsonl)
     t_start, budget_s = time.time(), float(os.environ.get("B2P_BENCH_EXPERIMENT_BUDGET_S", "270"))
     common = ["--steps", str(args.steps), "--warmup", str(args.warmup), "--order", str(args.order), "--n", str(args.n),
               "--no-cpu-baseline", "--no-experiments"]
@@ -388,8 +399,8 @@ def main():
     stream = torch.cuda.current_stream()
 
     qbytes = prob["local_ne"] * 10 * q1d ** 3 * 8
-    flush = torch.empty(256 * 1024 * 1024 // 8, dtype=torch.float64, device="cuda")  # > 126 MB L2
-    # B2P_BENCH_FLUSH=write_read (side experiment only): read the buffer back after writing it, so the 126 MB the flush
+    flush = torch.empty(256 * 1024 * 1024 // 8, dtype=torch.float64, device="cuda")  # > 50 MB L2 of an H100
+    # B2P_BENCH_FLUSH=write_read (side experiment only): read the buffer back after writing it, so the 50 MB the flush
     # leaves in L2 are CLEAN lines -- a plain write leaves them dirty and the timed kernels pay their write-back.
     flush_read = os.environ.get("B2P_BENCH_FLUSH", "write") == "write_read"
 
@@ -428,6 +439,7 @@ def main():
         b.record(stream)
     barrier()
     t_wall1 = time.time()
+    y_last = yd.cpu().numpy() if args.dump_outputs else None  # later legs reuse yd
     ms = np.array([a.elapsed_time(b) for a, b in evs])
     total_ms = float(ms.sum())
     clocks = sampler.stop(t_wall0, t_wall1) if sampler else None
@@ -456,15 +468,7 @@ def main():
         kernel_name = "nd_hex_apply6_kernel"
     elif forced in ("0", "7") and args.order in (4, 5, 6) and not args.assemble_qdata:
         kernel_name = "nd_hex_apply7_kernel"
-    traffic = None
-    try:  # DRAM bytes of the same kernel/launch shape from the committed ncu capture (profiles/)
-        with open(os.path.join(ROOT, "profiles", "r02_traffic.json")) as f:
-            tr = json.load(f)
-        if args.order == 3 and args.n == 29 and not args.assemble_qdata and world == 1:
-            k = tr[kernel_name + "<3,4,CURLCURL_MASS,geom>"]
-            traffic = k["dram_bytes_read"] + k["dram_bytes_write"]
-    except Exception:
-        pass
+    traffic = None  # DRAM bytes from hardware counters: not measured
     peak, peak_src = measured_peak_gbs()
     achieved = abytes / (k_ms * 1e-3) / 1e9
 
@@ -576,6 +580,8 @@ def main():
             except Exception as exc:
                 partition_parity = {"failed": f"{type(exc).__name__}: {str(exc)[:200]}"}
 
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, rank, y_last)
     line = None
     if rank == 0:
         line = {

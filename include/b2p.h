@@ -1,4 +1,4 @@
-/* b2p — B200-native (sm_100a) drop-in for Palace's partial-assembly operator path and the
+/* b2p — H100-native (sm_90a) drop-in for Palace's partial-assembly operator path and the
  * smoother / multigrid / Krylov loop that drives it.  Plain C ABI: opaque handles, raw pointers
  * and sizes, no C++/torch types.  Every entry point returns 0 on success or a non-zero code with
  * a message retrievable through b2p_last_error() (mirrors libCEED's CEED_ERROR_SUCCESS +
@@ -10,7 +10,7 @@
  * the caller owns all vectors; device vector pointers are only used in stream order of the call.
  * Threading: one caller thread per b2p_ctx (the reference uses exactly one Ceed context on GPU,
  * /root/reference/palace/fem/libceed/ceed.cpp:35-39). All work is enqueued on the stream given.
- * There is NO CPU fallback: every entry fails with B2P_ERR_CUDA when no sm_100 device is usable.
+ * There is NO CPU fallback: every entry fails with B2P_ERR_CUDA when no sm_90 device is usable.
  */
 #ifndef B2P_H
 #define B2P_H

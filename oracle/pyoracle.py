@@ -6,6 +6,7 @@ from __future__ import annotations
 import ctypes as C
 import os
 import subprocess
+import tempfile
 
 import numpy as np
 
@@ -35,14 +36,15 @@ def lib():
 
 
 def use_native_build():
-    """Timed CPU baseline only (bench.py): rebuild the oracle with -march=native ON THIS HOST into
-    oracle/_native/ and switch to it, so the baseline is not handicapped by the portable ISA level of the
-    prebuilt library. Returns True when the native build is in use."""
+    """Timed CPU baseline only (bench.py): rebuild the oracle with -march=native ON THIS HOST into a
+    temporary directory (never into the source tree) and switch to it, so the baseline is not handicapped by the
+    portable ISA level of the prebuilt library. Returns True when the native build is in use."""
     global _LIB
     try:
-        subprocess.check_call(["make", "-s", "-C", _HERE, "native"], stdout=subprocess.DEVNULL, stderr=subprocess.DEVNULL,
-                              timeout=300)
-        _LIB = C.CDLL(os.path.join(_HERE, "_native", "liboracle.so"))
+        out = tempfile.mkdtemp(prefix="b2p_oracle_native_")
+        subprocess.check_call(["make", "-s", "-C", _HERE, "native", f"NATIVE_DIR={out}"], stdout=subprocess.DEVNULL,
+                              stderr=subprocess.DEVNULL, timeout=300)
+        _LIB = C.CDLL(os.path.join(out, "liboracle.so"))
         _LIB.orc_nd_hex_ndof.restype = C.c_int
         return True
     except Exception:

@@ -1,9 +1,9 @@
-"""ctypes binding of the C ABI in include/b2p.h (libb2p.so, hand-written sm_100a kernels).
+"""ctypes binding of the C ABI in include/b2p.h (libb2p.so, hand-written sm_90a kernels).
 
 This is the only way Python reaches the product: there is no Python/NumPy/torch implementation of
 any operator behind it and no CPU fallback. Loading fails loudly when the library has not been
 built (``python -c 'import __graft_entry__ as g; g.build()'``) and every entry point fails when no
-sm_100 GPU is present. torch is used by the callers only to own device memory and streams.
+sm_90 GPU (H100) is present. torch is used by the callers only to own device memory and streams.
 """
 from __future__ import annotations
 
@@ -37,7 +37,7 @@ def lib():
     global _lib
     if _lib is None:
         if not os.path.exists(LIB_PATH):
-            raise B2PError(f"{LIB_PATH} not built: run __graft_entry__.build() (nvcc, sm_100a). No CPU fallback exists.")
+            raise B2PError(f"{LIB_PATH} not built: run __graft_entry__.build() (nvcc, sm_90a). No CPU fallback exists.")
         _lib = C.CDLL(LIB_PATH)
         _lib.b2p_last_error.restype = C.c_char_p
         _lib.b2p_last_error.argtypes = [C.c_void_p]

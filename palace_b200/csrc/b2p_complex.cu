@@ -24,7 +24,7 @@ using cplx = std::complex<double>;
 namespace
 {
 constexpr int NT = 256;
-constexpr int RED_BLOCKS = 296;
+constexpr int RED_BLOCKS = 264;  // two blocks per SM of an H100 SXM (132 SMs)
 constexpr int MAXM = 4;  // complex vectors per multi-dot pass
 
 struct CVecList
@@ -190,7 +190,7 @@ void cmulti_dot(b2p_ctx *c, int m, const CCPtr *V, CCPtr w, int64_t n, cplx *out
       L.re[j] = j < mm ? V[j0 + j].re : nullptr;
       L.im[j] = j < mm ? V[j0 + j].im : nullptr;
     }
-    const int rg = std::min(RED_BLOCKS, 2 * std::max(1, c->sm_count));  // two blocks per SM (296 on a B200)
+    const int rg = std::min(RED_BLOCKS, 2 * std::max(1, c->sm_count));  // two blocks per SM
     B2P_LAUNCH(cmulti_dot_kernel, rg, NT, 0, c->stream, L, w.re, w.im, n, mm, part);
     B2P_LAUNCH(creduce_kernel, 2 * mm, 32, 0, c->stream, part, rg, res);
     if (c->nranks > 1 && c->comm) b2p_allreduce_sum(c, res, 2 * mm);
@@ -309,9 +309,8 @@ public:
   // (operator.cpp:98-134) and streams the geometry once.
   void build_fused()
   {
-    // Default since round 2: measured on a B200 at 0.136 ms per complex matvec of K + lossy M + conductivity term on 2.02M
-    // complex dofs against 0.351 ms term by term (2.6x, profiles/r02_zfused_p3.json); parity with the term-by-term path in
-    // tests/test_zfused_gpu.py. B2P_COMPLEX_FUSED=0 keeps one real apply per term and part.
+    // Default: one pass over the geometry instead of one real apply per term and part (tools/zfused_bench.py times both);
+    // parity with the term-by-term path in tests/test_zfused_gpu.py. B2P_COMPLEX_FUSED=0 keeps one real apply per term and part.
     const char *env = std::getenv("B2P_COMPLEX_FUSED");
     if (env && env[0] == '0') return;
     const b2p_op *o0 = terms[0].op;

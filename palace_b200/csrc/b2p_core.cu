@@ -103,10 +103,10 @@ int apply_range(b2p_op *op, const int32_t *lidx, double alpha, const double *x, 
   if (op->kind == B2P_H1_DIFFUSION) return simple ? launch_h1_hex_apply(op, lidx, alpha, x, y, rg, s) : launch_h1_hex_apply3(op, lidx, alpha, x, y, rg, s);
   if (simple) return launch_nd_hex_apply(op, lidx, alpha, x, y, rg, s);
   // One-element-per-warp variant (p = 3, q1d = 4, mirror-symmetric tables): opt-in through the apply flag or
-  // B2P_ND_KERNEL=5; measured slower than nd_hex_apply4_kernel on B200 (DESIGN.md 4.1), kept for the analysis.
+  // B2P_ND_KERNEL=5; slower than nd_hex_apply4_kernel (DESIGN.md 4.1), kept for the analysis.
   // B2P_ND_KERNEL = 4 | 5 | 6 | 7 forces one of the sum-factorised ND kernels; default: the register-gather pipeline
-  // nd_hex_apply6_kernel where it is the faster one on B200 (p = 2, 3 at q1d = p + 1: 51.1 vs 54.6 us at p = 3, 78.5 vs 90.6 us
-  // at p = 2, profiles/r02_nd6_variants.txt), nd_hex_apply4_kernel everywhere else.
+  // nd_hex_apply6_kernel where it is the faster one (p = 2, 3 at q1d = p + 1; bench.py's round1_kernel_nd_hex_apply4 experiment
+  // times the alternative), nd_hex_apply4_kernel everywhere else.
   static const int nd_kernel = []
   {
     const char *e = std::getenv("B2P_ND_KERNEL");
@@ -121,8 +121,8 @@ int apply_range(b2p_op *op, const int32_t *lidx, double alpha, const double *x, 
     return launch_nd_hex_apply6(op, lidx, alpha, x, y, rg, s);
   }
   // p = 4, 5, 6 at q1d = p + 1: nd_hex_apply7_kernel (one CTA per element batch, warps specialised by vector component, one 1-D
-  // line per thread): 62.8 / 65.2 / 67.0 us against 73.6 / 114.9 / 232.6 us of nd_hex_apply4_kernel at 2.2-2.4M dofs
-  // (profiles/r02_nd7_component_barriers_ab.jsonl). B2P_ND_KERNEL=4 or B2P_APPLY_ROUND1_KERNEL select the round-1 kernel.
+  // line per thread; faster than nd_hex_apply4_kernel at these orders, tools/nd7_ab.py times both). B2P_ND_KERNEL=4 or
+  // B2P_APPLY_ROUND1_KERNEL select the round-1 kernel.
   if (((flags & B2P_APPLY_CTA_KERNEL) || nd_kernel == 7 || nd_kernel == 0) && !(flags & B2P_APPLY_ROUND1_KERNEL) && nd_hex_apply7_eligible(op))
   {
     static const bool trace = std::getenv("B2P_TRACE_KERNEL") != nullptr;
@@ -176,8 +176,9 @@ int b2p_ctx_create(int cuda_device, b2p_ctx **out)
   B2P_CUDA(nullptr, cudaSetDevice(cuda_device));
   cudaDeviceProp prop;
   B2P_CUDA(nullptr, cudaGetDeviceProperties(&prop, cuda_device));
-  B2P_CHECK(nullptr, prop.major >= 10, B2P_ERR_CUDA,
-            "b2p_ctx_create: device %d is sm_%d%d; this library is built for sm_100a only", cuda_device, prop.major,
+  // sm_90a code runs on compute capability 9.0 only: the arch-specific ("a") features have no forward compatibility
+  B2P_CHECK(nullptr, prop.major == 9 && prop.minor == 0, B2P_ERR_CUDA,
+            "b2p_ctx_create: device %d is sm_%d%d; this library is built for sm_90a only", cuda_device, prop.major,
             prop.minor);
   b2p_ctx *ctx = new b2p_ctx;
   ctx->device = cuda_device;

@@ -11,7 +11,7 @@
 //
 // issued as mma.sync.m8n8k4.f64 (SASS DMMA.8x8x4): A fragments stream from the (L2-resident) table,
 // B fragments from the element vectors in shared memory, the 8 elements of the batch are the N
-// dimension. tcgen05 has no FP64 kind, so DMMA is the tensor path for double precision on sm_100a.
+// dimension. wgmma has no FP64 kind, so DMMA is the tensor path for double precision on sm_90a.
 // The sum-factorised hex kernels (b2p_hex_nd3.cu) do the same operator in O(p^4) and are ~4x faster;
 // this kernel is the fallback that covers every other element type MFEM can describe by tables.
 #include <cstdlib>

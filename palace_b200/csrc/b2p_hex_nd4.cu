@@ -2,7 +2,7 @@
 //
 //   y_L += alpha * sum_e E_e^T  B^T  D  B  E_e x_L          (curl-curl, mass, curl-curl + mass)
 //
-// Same operator as b2p_hex_nd.cu (the simple cross-check kernel), organised for the B200:
+// Same operator as b2p_hex_nd.cu (the simple cross-check kernel), organised as:
 //   * persistent grid; every WARP owns a batch of NEW elements through all five phases, so the only
 //     synchronisation is __syncwarp() (no CTA barriers, warps drift apart and fill each other's stalls):
 //       Z   z-contraction of the gathered dofs          (reads the staged x values)

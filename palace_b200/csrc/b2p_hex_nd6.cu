@@ -55,7 +55,7 @@ struct ND6Params
   // 1-D tables, rows c < H = ceil(q/2) only: the launcher has verified the mirror symmetry of MFEM's Gauss-Legendre /
   // Gauss-Lobatto bases on a symmetric point set, Bo[q-1-c][p-1-i] = Bo[c][i], Bc[q-1-c][n-1-i] = Bc[c][i],
   // Gc[q-1-c][n-1-i] = -Gc[c][i]. ptxas keeps every table entry a DFMA touches in a REGISTER (no constant-bank operand
-  // on the FP64 pipe of sm_100a: 0 of 924 DFMA in the round-1 SASS), so half the rows is 40 registers less.
+  // on the FP64 pipe: 0 of 924 DFMA in the round-1 SASS), so half the rows is 40 registers less.
   static constexpr int H = (Q_ + 1) / 2;
   double Bo[H * P_];
   double Bc[H * (P_ + 1)];

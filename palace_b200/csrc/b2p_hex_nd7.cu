@@ -726,26 +726,25 @@ __global__ void __launch_bounds__(3 * WPC * 32, MINB) nd_hex_apply7_kernel(const
 }
 
 // Launch shape per order: elements per batch, warps per component, CTAs per SM (register cap 65536 / threads per SM), q-data
-// staged by TMA, component-wide barriers. Times: 2.2-2.4M dofs on one B200, L2 flushed (profiles/r02_nd7_shapes_ab.jsonl,
-// r02_nd7_component_barriers_ab.jsonl; tools/nd7_ab.py).
+// staged by TMA, component-wide barriers; chosen by A/B timing of the shapes (tools/nd7_ab.py, B2P_ND7_CFG).
 template <int P_>
 struct ND7Shape;
 template <>
 struct ND7Shape<4>
 {
-  static constexpr int NE = 1, WPC = 1, MINB = 8;  // 25 of 32 lanes, 96 threads: 62.8 us (CTA barriers 63.9, LDG q-data 69.2, nd_hex_apply4_kernel 73.6)
+  static constexpr int NE = 1, WPC = 1, MINB = 8;  // 25 of 32 lanes, 96 threads
   static constexpr bool GSM = true, CBAR = true;
 };
 template <>
 struct ND7Shape<5>
 {
-  static constexpr int NE = 2, WPC = 3, MINB = 2;  // 72 of 96 lanes, 288 threads: 65.2 us (CTA barriers 65.7, LDG q-data 75.8, nd_hex_apply4_kernel 114.9)
+  static constexpr int NE = 2, WPC = 3, MINB = 2;  // 72 of 96 lanes, 288 threads
   static constexpr bool GSM = true, CBAR = true;
 };
 template <>
 struct ND7Shape<6>
 {
-  static constexpr int NE = 1, WPC = 2, MINB = 3;  // 49 of 64 lanes, 192 threads: 67.0 us (CTA barriers 67.2, LDG q-data 73.8, nd_hex_apply4_kernel 232.6)
+  static constexpr int NE = 1, WPC = 2, MINB = 3;  // 49 of 64 lanes, 192 threads
   static constexpr bool GSM = true, CBAR = true;
 };
 

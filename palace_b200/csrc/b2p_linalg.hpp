@@ -1,4 +1,4 @@
-// Device-resident linear algebra and solver layer (C++ host logic over sm_100a kernels), mirroring
+// Device-resident linear algebra and solver layer (C++ host logic over sm_90a kernels), mirroring
 // the reference's class structure so that the C ABI (and a Palace adapter) maps one to one:
 //   palace::Operator / ParOperator / SumOperator        /root/reference/palace/linalg/{operator.hpp,rap.hpp}
 //   palace::Solver<OperType>                            /root/reference/palace/linalg/solver.hpp:21-65

@@ -98,8 +98,8 @@ void ParOperator::MultHaloBody(const double *x, double *y, cudaStream_t s) const
   //   zero y and y_ghost; forward exchange (P); all elements; reverse exchange (P^T) + add into y.
   // With peer mailboxes (b2p_halo_p2p_*) the exchanges are NVLink stores + flags issued from small
   // kernels on this stream; otherwise NCCL grouped send/recv. (An interior/interface split that overlaps
-  // the collectives with the element kernel was measured to give nothing on B200: the persistent element
-  // kernel fills every SM, so a collective kernel launched beside it only starts when it retires.)
+  // the collectives with the element kernel gives nothing: the persistent element kernel fills every SM, so a
+  // collective kernel launched beside it only starts when it retires.)
   Halo *h = halo;
   // B2P_HALO_TIMING=1 (diagnostic): CUDA events between the three launches, accumulated per operator and printed by the
   // destructor -- where the time of a partitioned Mult goes on this rank (the events serialise nothing: same stream).
@@ -192,8 +192,7 @@ void ParOperator::Mult(const double *x, double *y) const
   {
     // Zero-fill by a kernel that releases its dependent at once, first element kernel launched with programmatic stream
     // serialisation: its prologue and first batch overlap the zero-fill (it waits on the grid dependency just before its
-    // first scatter). Measured on B200: 54.9 vs 55.6 us per Mult at 2.02M dofs (profiles/r02_nd6_variants.txt); B2P_PDL=0
-    // goes back to memset + plain launch.
+    // first scatter). B2P_PDL=0 goes back to memset + plain launch (bench.py times both).
     static const bool pdl = []() { const char *e = getenv("B2P_PDL"); return !(e && e[0] == '0'); }();
     const b2p_op *o0 = terms[0].op;
     const bool pdl_ok = pdl && !o0->dense && o0->kind != B2P_H1_DIFFUSION && o0->lidx_bc != nullptr;
@@ -220,8 +219,8 @@ void ParOperator::Mult(const double *x, double *y) const
     // Capture and replay on an internal BLOCKING stream instead -- it synchronises implicitly with the legacy stream in
     // both directions, so the caller's ordering is preserved. (B2P_GRAPH_STREAM=0: a legacy-stream context runs the eager
     // sequence, as in round 1.)
-    // Measured on 2 B200s (profiles/r02_bench_2gpu_halo_variants.json): replay on the internal blocking stream costs more in
-    // legacy-stream synchronisation than it saves in launches (81.4 vs 78.4 us per Mult) -- opt-in, B2P_GRAPH_STREAM=1.
+    // Replay on the internal blocking stream can cost more in legacy-stream synchronisation than it saves in launches
+    // -- opt-in, B2P_GRAPH_STREAM=1.
     static const bool graph_stream = []() { const char *e = getenv("B2P_GRAPH_STREAM"); return e && e[0] == '1'; }();
     if (s == nullptr && graph_stream && !no_graph)
     {

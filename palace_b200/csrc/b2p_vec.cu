@@ -91,7 +91,7 @@ __device__ __forceinline__ void block_reduce_store(double (&acc)[M], double *out
   }
 }
 
-constexpr int RED_BLOCKS = 296;  // 2 x 148 SMs; fixed so the summation order is reproducible
+constexpr int RED_BLOCKS = 264;  // 2 x 132 SMs (H100 SXM, the most of any sm_90 part); fixed so the summation order is reproducible
 constexpr int MAXM = 8;          // vectors per multi-dot pass
 
 struct VecList
@@ -158,7 +158,7 @@ __host__ __device__ __forceinline__ uint64_t splitmix64(uint64_t x)
 }
 
 // Partial sums of m dot products live in ctx->d_red: [MAXM][RED_BLOCKS] partials then [MAXM] results.
-// Blocks of a reduction pass: two per SM (296 on a B200), fixed per device so the summation order is reproducible.
+// Blocks of a reduction pass: two per SM (264 on an H100 SXM), fixed per device so the summation order is reproducible.
 int red_grid(b2p_ctx *c) { return std::min(RED_BLOCKS, 2 * std::max(1, c->sm_count)); }
 double *red_partials(b2p_ctx *c) { return c->d_red; }
 double *red_results(b2p_ctx *c) { return c->d_red + (size_t)MAXM * RED_BLOCKS; }

@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run with -m gpu under gpurun)")
+    config.addinivalue_line("markers", "gpu: needs a real H100 (sm_90a; run with -m gpu)")
     if os.environ.get("B2P_EMU_TESTS") == "1":
         # pre-GPU validation: the same tests against the host-thread SIMT emulation build of the kernel sources
         from tests.emu import emu_mode

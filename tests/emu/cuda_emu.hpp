@@ -9,7 +9,7 @@
 // "device" allocations are poisoned. Fibers of a barrier interval run one after the other (order selectable with
 // B2P_EMU_ORDER=fwd|rev|rand), so a missing barrier between a producer and a consumer phase shows up as stale
 // data for some lane order. Blocks run one at a time. This validates indexing, data flow, synchronisation protocol
-// and arithmetic of a kernel before it is run on a B200; it says nothing about performance. The product never
+// and arithmetic of a kernel before it is run on an H100; it says nothing about performance. The product never
 // links or loads it: B2P_EMU is defined only by tests/emu/Makefile.
 #pragma once
 #include <sys/mman.h>

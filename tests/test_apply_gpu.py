@@ -1,4 +1,4 @@
-"""GPU parity: the sm_100a sum-factorised kernels (through the C ABI) against the dense
+"""GPU parity: the sm_90a sum-factorised kernels (through the C ABI) against the dense
 reference-style CPU oracle on the same seeded inputs. Mirrors the structure of the reference's
 "3D libCEED Operators" tests (/root/reference/test/unit/test-libceed.cpp:245-376,749-806): Mult,
 diagonal; meshes with rotated element frames, curved (order-2) geometry, striped piecewise

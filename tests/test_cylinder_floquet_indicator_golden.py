@@ -1,5 +1,5 @@
 """End-to-end comparison of the COMPLEX post-processing chain of a Floquet run with the reference's own output (CPU, oracle side;
-slow: B2P_SLOW_TESTS=1, output kept in profiles/r02_floquet_indicator_vs_reference.log): error-indicators.csv of
+slow: B2P_SLOW_TESTS=1): error-indicators.csv of
 examples/cylinder/floquet.json. For each of the 15 complex modes of the Hermitian pencil of test_cylinder_floquet_golden.py:
     B = -1/(i w) curl E + (1/w) M_rt^-1 ([k x] E, v)      (drivers/eigensolver.cpp:470-482, linalg/floquetcorrection.cpp)
     eta_K^2 = (grad-flux + curl-flux element errors of the real and of the imaginary parts) * 0.5 / (E_elec + E_mag)

@@ -1,5 +1,5 @@
 """End-to-end comparison of the flux error estimators on TETRAHEDRA with the reference's own output (CPU, oracle side; slow: runs
-only with B2P_SLOW_TESTS=1, its output is kept in profiles/r02_tet_indicator_vs_reference.log): error-indicators.csv of
+only with B2P_SLOW_TESTS=1): error-indicators.csv of
 examples/cylinder/waveguide.json -- the periodic tetrahedral waveguide of test_cylinder_tet_golden.py, Nedelec order 4, 15 modes,
 grad-flux + curl-flux estimators -- against oracle/estimator.py on the oracle-side tet discretisation: ND_4 with its curl-oriented
 transformations, RT_3 (tetspace.build_rt_tet_space), the element-local discrete curl, quadratic geometry.

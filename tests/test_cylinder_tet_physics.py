@@ -3,40 +3,39 @@ example on its tetrahedral mesh (/root/reference/examples/cylinder/mesh/cylinder
 order-3 ND tet discretisation (element tables, curl-oriented restrictions of arbitrarily ordered neighbours, order-2 geometry
 q-data) must give the closed-form TM/TE frequencies of docs/src/examples/cylinder.md:36-120 to discretisation accuracy, with
 the doubly degenerate modes degenerate to round-off -- which fails for any conformity / orientation error on shared faces.
+The mesh is the one stored in tests/golden/cylinder_waveguide_tet.npz (tests/golden/make_cylinder_tet_fixture.py).
 (The reference stores regression output for the hexahedral mesh only; that one is pinned in tests/test_cylinder_golden.py.)"""
 import os
 
 import numpy as np
-import pytest
 import scipy.sparse as sp
 import scipy.sparse.linalg as spla
 
 from oracle import pyoracle as O
 from palace_b200.host import coeff as cf
-from palace_b200.host import gmsh
 from palace_b200.host import tetspace as ts
 
-MESH = "/root/reference/examples/cylinder/mesh/cylinder_tet.msh"
+MESH = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "cylinder_waveguide_tet.npz")
 # cylinder.md table (GHz): TM010, TE111 (x2), TM011, TE211 (x2), TE112 (x2)
 ANALYTIC = np.array([2.903605, 2.922212, 2.922212, 3.468149, 4.146842, 4.146842, 4.396673, 4.396673])
 
 
-@pytest.mark.skipif(not os.path.exists(MESH), reason="needs the reference's example mesh")
 def test_tet_cylinder_cavity_frequencies():
-    m = gmsh.load_tets(MESH)
-    assert m.order == 2
+    m = np.load(MESH)
+    assert int(m["geom_order"]) == 2
     p = 3
-    mesh = ts.TetMesh(m.verts, m.elems, m.attr)
+    ne = m["elems"].shape[0]
+    mesh = ts.TetMesh(m["verts"], m["elems"], m["attr"])
     nd = ts.build_nd_tet_space(mesh, p)
     interp, curl, qpts, qw = ts.nd_tet_tables(p, 2 * p + 2)
-    qd = ts.geom_qdata(m.xe, np.ones(m.ne, dtype=np.int32), m.order, qpts, qw)
+    qd = ts.geom_qdata(m["xe"], np.ones(ne, dtype=np.int32), 2, qpts, qw)
     assert (qd[:, 1, :] > 0).all() and abs(qd[:, 1, :].sum() / (np.pi * 2.74 ** 2 * 5.48) - 1) < 5e-4
     one = cf.coeff_ctx(a=1.0)
 
     def assemble(kind):
         Ae = O.element_matrices(kind, interp, curl, None, qd, one, nd.P)
         rows, cols, vals = [], [], []
-        for e in range(m.ne):
+        for e in range(ne):
             T = nd.dense_T(e)
             r, c = np.meshgrid(nd.idx[e], nd.idx[e], indexing="ij")
             rows.append(r.ravel())

@@ -1,8 +1,7 @@
 """CPU: pins the oracle's restated pointwise arithmetic (geometry factors, D for hcurl / hdiv /
 hdivmass) to golden vectors produced by the REFERENCE's own QFunction headers
-(tests/golden/make_golden.py; /root/reference/palace/fem/qfunctions/33/*.h), and -- when oracle/_ref
-is present -- to the compiled reference directly."""
-import ctypes as C
+(tests/golden/make_golden.py; the reference's palace/fem/qfunctions/33/*.h), including the compiled reference's outputs
+on the inputs of test_against_compiled_reference_headers (tests/golden/qf_direct_golden.npz)."""
 import os
 
 import numpy as np
@@ -64,17 +63,15 @@ def test_build_qfunctions_are_consistent_with_apply():
     assert _rel(np.einsum("rcq,cq->rq", G["build_hdiv"].reshape(3, 3, -1, order="F"), c), G["hdiv_w"]) < 1e-14
 
 
-@pytest.mark.skipif(O.ref() is None, reason="oracle/_ref not built (no /root/reference on this box)")
 def test_against_compiled_reference_headers():
-    ref = O.ref()
+    """f_apply_hdivmass_33 of the compiled reference on these inputs, stored by tests/golden/make_golden.py direct."""
+    ref = np.load(os.path.join(os.path.dirname(__file__), "golden", "qf_direct_golden.npz"))
     rng = np.random.default_rng(7)
     Q = 40
-    p = lambda a: a.ctypes.data_as(C.c_void_p)
     qdata = np.ascontiguousarray(G["qdata"][:, :Q])
     u, c = rng.random((3, Q)), rng.random((3, Q))
-    v, w = np.empty((3, Q)), np.empty((3, Q))
+    v, w = ref["hdivmass_v"], ref["hdivmass_w"]
     ctx = np.ascontiguousarray(G["ctx_pair"])
-    assert ref.ref_apply_hdivmass_33(p(ctx), Q, p(qdata), p(u), p(c), p(v), p(w)) == 0
     vo, wo = O.apply_D(O.CURLCURL_MASS, ctx, qdata, u, c)
     assert _rel(vo, v) < TOL and _rel(wo, w) < TOL
 

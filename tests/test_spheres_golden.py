@@ -1,13 +1,15 @@
 """END-TO-END pin of the TETRAHEDRAL geometry / space path against numbers produced by the reference itself: the
 capacitance matrix of the two-spheres electrostatics example (/root/reference/examples/spheres/spheres.json: 14,362
 curved cubic tetrahedra TET20, H1 order 3, 66,328 dofs) that Palace's regression suite stores in
-test/data/regression/ref/spheres/terminal-C.csv. The oracle-side path -- Gmsh reader (palace_b200/host/gmsh.py), order-3
+test/data/regression/ref/spheres/terminal-C.csv. The oracle-side path -- order-3
 tet geometry q-data and the H1 tet space of palace_b200/host/tetspace.py, the reference QFunction arithmetic of the oracle,
 a Jacobi-preconditioned CG solve to 1e-13 -- reproduces all four entries to 1.4e-10 relative when the forms are integrated with the rule
 the reference uses (q_order = 2 p = 6 -> the 24-point symmetric rule, tetspace.tet_quadrature_symmetric6); with the 64-point conical
 rule of the same degree the entries sit 4e-8 ... 7e-8 away: on curved elements the integrand is not a polynomial, and the choice of
-rule is what round 1's looser pin was seeing. The remaining 1.3e-10 is uniform over the four entries (the physical constants' digits). The mesh is read from the reference tree (3.4 MB, not copied
-into this repository), so the test runs only where /root/reference exists.
+rule is what round 1's looser pin was seeing. The remaining 1.3e-10 is uniform over the four entries (the physical constants' digits). The mesh
+(examples/spheres/mesh/spheres.msh of the reference, 3.4 MB) is stored in tests/golden/spheres_mesh.npz as its corners, connectivity
+and the nodes that sit off the affine image of their element's corners (tests/golden/make_spheres_fixture.py); every other node is
+rebuilt here from the corners.
 
 The same run's error-indicators.csv pins the GRAD-FLUX estimator on these curved tetrahedra (GradFluxErrorEstimator,
 /root/reference/palace/linalg/errorestimator.cpp:272-398 and drivers/electrostaticsolver.cpp:77-86): E = -grad V in ND_3 by the element-local
@@ -28,7 +30,7 @@ from palace_b200.host import coeff as cf
 from palace_b200.host import gmsh
 from palace_b200.host import tetspace as ts
 
-MESH = "/root/reference/examples/spheres/mesh/spheres.msh"
+MESH = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "spheres_mesh.npz")
 RULE = ts.tet_quadrature_symmetric6
 # test/data/regression/ref/spheres/terminal-C.csv (farads)
 # test/data/regression/ref/spheres/error-indicators.csv: Norm, Minimum, Maximum, Mean
@@ -36,9 +38,26 @@ IND_REF = (6.910139872411e-03, 1.217546964778e-06, 5.028157468369e-04, 3.3831235
 C_REF = np.array([[+1.237445610357e-12, -4.770975738888e-13], [-4.770975738888e-13, +2.478413459856e-12]])
 
 
+def affine_nodes(verts, elems, order):
+    """[ne][Nn][3]: the lattice points of gmsh.load_tets's node order mapped by each element's affine corner map."""
+    lat = np.array([(a, b, c) for c in range(order + 1) for b in range(order + 1 - c) for a in range(order + 1 - b - c)], dtype=np.float64) / order
+    V = verts[elems]
+    return V[:, :1] + np.einsum("nd,edc->enc", lat, V[:, 1:] - V[:, :1])
+
+
+def load_fixture(path):
+    z = np.load(path)
+    order, verts, elems = int(z["order"]), z["verts"], z["elems"].astype(np.int64)
+    X = affine_nodes(verts, elems, order)
+    e, n = np.nonzero(z["curved_idx"] >= 0)                          # nodes off their affine positions (-1: affine)
+    X[z["curved"][e], n] = z["curved_nodes"][z["curved_idx"][e, n]]
+    return gmsh.HighOrderTetMesh(order, verts, elems, z["attr"], np.ascontiguousarray(np.transpose(X, (0, 2, 1))), z["bdr_attr"],
+                                 z["bdr_verts"].astype(np.int64))
+
+
 @pytest.fixture(scope="module")
 def spheres():
-    m = gmsh.load_tets(MESH)
+    m = load_fixture(MESH)
     assert m.order == 3 and m.ne == 14362
     p = 3                                                            # spheres.json "Order": 3
     mesh = ts.TetMesh(m.verts, m.elems, m.attr)
@@ -84,7 +103,6 @@ def spheres():
     return dict(m=m, mesh=mesh, nd=nd, h1=h1, p=p, qpts=qpts, qd=qd, K=K, V=V)
 
 
-@pytest.mark.skipif(not os.path.exists(MESH), reason="needs the reference's example mesh")
 def test_capacitance_matrix_of_the_spheres_example(spheres):
     K, V = spheres["K"], spheres["V"]
     mu0, c0, L0 = 1.25663706127e-6, 299792458.0, 1.0e-2              # palace/utils/constants.hpp:22-30, "L0": 1e-2
@@ -94,7 +112,6 @@ def test_capacitance_matrix_of_the_spheres_example(spheres):
     assert rel.max() < 1e-9
 
 
-@pytest.mark.skipif(not os.path.exists(MESH), reason="needs the reference's example mesh")
 def test_error_indicators_of_the_spheres_example(spheres):
     """Vectorised over the 14,362 elements (the oracle's per-point loops, oracle/estimator.py, are held to it on a handful of them)."""
     m, mesh, nd, h1, p, qpts, qd, K = (spheres[k] for k in ("m", "mesh", "nd", "h1", "p", "qpts", "qd", "K"))
@@ -144,7 +161,6 @@ def test_error_indicators_of_the_spheres_example(spheres):
     assert abs(rel[0]) < 1e-6 and abs(rel[3]) < 1e-6 and abs(rel[1]) < 5e-4 and abs(rel[2]) < 1e-4
 
 
-@pytest.mark.skipif(not os.path.exists(MESH), reason="needs the reference's example mesh")
 def test_probe_field_of_the_spheres_example(spheres):
     """probe-E.csv: E = -grad V at (-1.49, 0, 0) cm, "just above the surface of the smaller sphere", for both terminals. The point is
     located in its curved cubic tetrahedron by Newton's method on the order-3 geometry map, E = -J^-T grad_ref V there; volts per metre
@@ -177,7 +193,6 @@ def test_probe_field_of_the_spheres_example(spheres):
         assert abs(Ev[0] / ref[k, 0] - 1) < 5e-7 and np.linalg.norm(Ev - ref[k]) < 2e-6 * np.linalg.norm(ref[k])
 
 
-@pytest.mark.skipif(not os.path.exists(MESH), reason="needs the reference's example mesh")
 def test_surface_charges_of_the_spheres_example(spheres):
     """surface-F.csv: the electric flux through each sphere for each terminal's field, Q = int eps E . n dS with n pointing into the
     domain, integrated on the CURVED boundary triangles -- each as a face of its parent cubic tetrahedron: points on the reference

@@ -1,8 +1,9 @@
 // Micro-benchmark (round 2, multi-GPU analysis): how long does a zero-fill of an 8 / 16 MB vector take right after the
-// bench's L2 flush (a 256 MB memset that leaves 126 MB of DIRTY lines in L2) compared with a clean L2?
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o zero_ubench zero_ubench.cu && ./zero_ubench
+// bench's L2 flush (a 256 MB memset that leaves the 50 MB L2 of an H100 full of DIRTY lines) compared with a clean L2?
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o zero_ubench zero_ubench.cu && ./zero_ubench
 #include <cstdio>
 #include <cuda_runtime.h>
+constexpr int SMS = 132;  // H100 SXM
 __global__ void zero_kernel(double2 *y, long long n2)
 {
   const long long stride = (long long)gridDim.x * blockDim.x;
@@ -27,14 +28,14 @@ int main()
   cudaEventCreate(&b);
   for (int mode = 0; mode < 4; mode++)          // 0: dirty L2 (memset flush), 1: flush written then read back (clean L2), 2: no flush, 3: dirty, cudaMemsetAsync
     for (int mb = 8; mb <= 16; mb *= 2)
-      for (int grid = 148 * 2; grid <= 148 * 8; grid *= 2)
+      for (int grid = SMS * 2; grid <= SMS * 8; grid *= 2)
       {
         float tot = 0.f;
         const int reps = 20;
         for (int r = 0; r < reps + 2; r++)
         {
           if (mode != 2) cudaMemsetAsync(flush, 0, NF);
-          if (mode == 1) read_kernel<<<148 * 8, 256>>>((const double2 *)flush, NF / 16, out);
+          if (mode == 1) read_kernel<<<SMS * 8, 256>>>((const double2 *)flush, NF / 16, out);
           cudaEventRecord(a);
           if (mode == 3)
             cudaMemsetAsync(y, 0, (size_t)mb << 20);

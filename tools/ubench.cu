@@ -1,5 +1,5 @@
 // Micro-benchmarks that size the kernel design: FP64 FMA vs DMMA (mma.sync m8n8k4 f64) issue
-// rate, mixed, shared-memory bandwidth, and fp64 atomic (RED) throughput. Build: nvcc -arch=sm_100a.
+// rate, mixed, shared-memory bandwidth, and fp64 atomic (RED) throughput. Build: nvcc -arch=sm_90a.
 #include <cstdio>
 #include <cuda_runtime.h>
 #include <vector>
