@@ -45,8 +45,10 @@ enum
   B2P_ND_MASS = 1,       /* VectorFEMassIntegrator    -> f_apply_hcurl_33     (integ/vecfemass.cpp:72-105)   */
   B2P_CURLCURL_MASS = 2, /* CurlCurlMassIntegrator    -> f_apply_hdivmass_33  (integ/curlcurlmass.cpp:37-44) */
   B2P_H1_DIFFUSION = 3,  /* DiffusionIntegrator       -> f_apply_hcurl_33 on grad (integ/diffusion.cpp:37-42) */
-  /* The Floquet-periodic terms on one ND space (models/spaceoperator.cpp:305-309); NOT symmetric; dense-basis operators only
-   * (b2p_op_create_dense with both tables; hexahedra enter with their dense tables). One coefficient context each, built by the
+  /* The Floquet-periodic terms on one ND space (models/spaceoperator.cpp:305-309); NOT symmetric (their transpose is applied with
+   * B2P_APPLY_TRANSPOSE). Dense-basis operators (b2p_op_create_dense with both tables) on any element, and sum-factorised
+   * operators on hexahedra (b2p_op_create, on-the-fly coefficients only: assemble_qdata = 1 returns B2P_ERR_UNSUPPORTED). On
+   * hexahedra they also fuse with curl-curl / mass terms in b2p_op_create_sum. One coefficient context each, built by the
    * caller as the reference's integrators do (PopulateCoefficientContext with a = -1 for the weak curl, transpose for the curl): */
   B2P_ND_WEAKCURL = 4,   /* MixedVectorWeakCurlIntegrator: values -> curls,  f_apply_hcurlhdiv_33 (integ/mixedveccurl.cpp:68-117) */
   B2P_ND_MIXEDCURL = 5   /* MixedVectorCurlIntegrator:     curls  -> values, f_apply_hdivhcurl_33 (integ/mixedveccurl.cpp:23-66)  */

@@ -135,7 +135,8 @@ inline b2p_geom *CreateHexGeometry(b2p_ctx *ctx, const mfem::Mesh &mesh, const m
   return geom;
 }
 
-// One integrator of the form on one hexahedral block: kind from fem/integ/{curlcurl,vecfemass,curlcurlmass}.cpp, the
+// One integrator of the form on one hexahedral block: kind from fem/integ/{curlcurl,vecfemass,curlcurlmass}.cpp, or one of
+// the Floquet pair of fem/integ/mixedveccurl.cpp (B2P_ND_WEAKCURL / B2P_ND_MIXEDCURL, on-the-fly coefficients only), the
 // coefficient context bytes exactly as PopulateCoefficientContext builds them (fem/libceed/coefficient.cpp:51-130).
 inline b2p_op *CreateHexNDIntegrator(b2p_ctx *ctx, b2p_geom *geom, int kind, const HexNDSpaceInputs &in, const void *coeff_ctx,
                                      size_t coeff_ctx_bytes, bool assemble_q_data = false)

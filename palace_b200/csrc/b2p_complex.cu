@@ -314,11 +314,14 @@ public:
     const char *env = std::getenv("B2P_COMPLEX_FUSED");
     if (env && env[0] == '0') return;
     const b2p_op *o0 = terms[0].op;
-    if (o0->dense && terms.size() >= 2)
+    bool block = false;
+    for (auto &t : terms) block = block || (!t.op->dense && t.op->bcoef);
+    if ((o0->dense || block) && terms.size() >= 2)
     {
       // Dense-basis terms (tets, prisms) have no complex element kernel; their sum still collapses to TWO real dense operators,
       // S_re = sum_t c_t^r A_t and S_im = sum_t c_t^i A_t (b2p_op_create_sum: stacked tables, summed per-element tensors), so a
-      // complex matvec costs 4 dense applies (2 when every c_t^i = 0) instead of 2-4 per term.
+      // complex matvec costs 4 dense applies (2 when every c_t^i = 0) instead of 2-4 per term. Sum-factorised hex terms with a
+      // mixed curl kind (Floquet-periodic models) take the same route: S_re and S_im are then two block operators.
       std::vector<b2p_op *> ops;
       std::vector<double> cr, ci;
       for (auto &t : terms)
@@ -338,7 +341,7 @@ public:
     for (auto &t : terms)
     {
       const b2p_op *o = t.op;
-      if (!nd_hex_apply4z_eligible(o) || o->geom != o0->geom || o->p != o0->p || o->q1d != o0->q1d || o->ne != o0->ne ||
+      if (!nd_hex_apply4z_eligible(o) || o->bcoef || o->geom != o0->geom || o->p != o0->p || o->q1d != o0->q1d || o->ne != o0->ne ||
           o->lsize != o0->lsize || o->PS != o0->PS || !o->ecoef || !o->lidx_bc)
         return;
     }
@@ -462,15 +465,17 @@ public:
         any_im = any_im || t.ci != 0.0;
       }
       const double si = herm ? -alpha : alpha;
+      // Z^H = S_re^T - i S_im^T: the transpose flag matters for block sums only (dense sums are symmetric)
+      const int fl = B2P_APPLY_MASKED | (herm ? B2P_APPLY_TRANSPOSE : 0);
       if (any_re)
       {
-        b2p_op_apply_add_ex(sum_re, alpha, x.re, y.re, B2P_APPLY_MASKED, s);
-        b2p_op_apply_add_ex(sum_re, alpha, x.im, y.im, B2P_APPLY_MASKED, s);
+        b2p_op_apply_add_ex(sum_re, alpha, x.re, y.re, fl, s);
+        b2p_op_apply_add_ex(sum_re, alpha, x.im, y.im, fl, s);
       }
       if (any_im)
       {
-        b2p_op_apply_add_ex(sum_im, -si, x.im, y.re, B2P_APPLY_MASKED, s);
-        b2p_op_apply_add_ex(sum_im, si, x.re, y.im, B2P_APPLY_MASKED, s);
+        b2p_op_apply_add_ex(sum_im, -si, x.im, y.re, fl, s);
+        b2p_op_apply_add_ex(sum_im, si, x.re, y.im, fl, s);
       }
       n_fused_applies++;
     }
@@ -478,15 +483,16 @@ public:
     for (auto &t : terms)
     {
       const double ci = herm ? -t.ci : t.ci;
+      const int fl = B2P_APPLY_MASKED | (herm ? B2P_APPLY_TRANSPOSE : 0);  // (only the non-symmetric kinds look at the flag)
       if (t.cr != 0.0)
       {
-        b2p_op_apply_add_ex(t.op, alpha * t.cr, x.re, y.re, B2P_APPLY_MASKED, s);
-        b2p_op_apply_add_ex(t.op, alpha * t.cr, x.im, y.im, B2P_APPLY_MASKED, s);
+        b2p_op_apply_add_ex(t.op, alpha * t.cr, x.re, y.re, fl, s);
+        b2p_op_apply_add_ex(t.op, alpha * t.cr, x.im, y.im, fl, s);
       }
       if (ci != 0.0)
       {
-        b2p_op_apply_add_ex(t.op, -alpha * ci, x.im, y.re, B2P_APPLY_MASKED, s);
-        b2p_op_apply_add_ex(t.op, alpha * ci, x.re, y.im, B2P_APPLY_MASKED, s);
+        b2p_op_apply_add_ex(t.op, -alpha * ci, x.im, y.re, fl, s);
+        b2p_op_apply_add_ex(t.op, alpha * ci, x.re, y.im, fl, s);
       }
     }
   }
@@ -541,7 +547,8 @@ private:
   int32_t *d_ess = nullptr;
   // fused complex element operator (build_fused)
   bool fused = false, fused_imag = false;
-  b2p_op *sum_re = nullptr, *sum_im = nullptr;  // dense-basis terms: the real and imaginary coefficient sums as two dense operators
+  // the real and imaginary coefficient sums as two operators: dense-basis terms, or hex terms with a mixed curl kind (block sums)
+  b2p_op *sum_re = nullptr, *sum_im = nullptr;
   int fused_kind = 0;
   double *zcoef = nullptr, *zcoef_h = nullptr;
   std::vector<std::vector<double>> fused_e18;  // host copies of the terms' per-element material tensors

@@ -99,6 +99,22 @@ int apply_range(b2p_op *op, const int32_t *lidx, double alpha, const double *x, 
                 cudaStream_t s)
 {
   if (op->dense) return launch_dense_apply(op, lidx, alpha, x, y, rg, s, (flags & B2P_APPLY_TRANSPOSE) != 0);
+  // Block operators (mixed curl kinds on hexes and sums containing one): nd_hex_apply6_kernel (p = 2, 3) or
+  // nd_hex_apply7_kernel (p = 4, 5, 6) at q1d = p + 1 with mirror-symmetric tables, the cross-check kernel for everything else
+  // and whenever an apply flag asks for another kernel (there is no block form in nd_hex_apply4/5_kernel).
+  if (op->bcoef)
+  {
+    const bool tr = (flags & B2P_APPLY_TRANSPOSE) != 0;
+    static const int forced = []
+    {
+      const char *e = std::getenv("B2P_ND_KERNEL");
+      return e ? std::atoi(e) : 0;
+    }();
+    const bool other = (flags & (B2P_APPLY_SIMPLE_KERNEL | B2P_APPLY_ROUND1_KERNEL | B2P_APPLY_HALFWARP_KERNEL)) || forced == 4 || forced == 5;
+    if (!other && nd_hex_apply6_eligible(op)) return launch_nd_hex_apply6(op, lidx, alpha, x, y, rg, s, tr);
+    if (!other && nd_hex_apply7_eligible(op)) return launch_nd_hex_apply7(op, lidx, alpha, x, y, rg, s, tr);
+    return launch_nd_hex_apply(op, lidx, alpha, x, y, rg, s, tr);
+  }
   const bool simple = flags & B2P_APPLY_SIMPLE_KERNEL;
   if (op->kind == B2P_H1_DIFFUSION) return simple ? launch_h1_hex_apply(op, lidx, alpha, x, y, rg, s) : launch_h1_hex_apply3(op, lidx, alpha, x, y, rg, s);
   if (simple) return launch_nd_hex_apply(op, lidx, alpha, x, y, rg, s);
@@ -367,6 +383,28 @@ bool decode_ctx(const IntScalar *c, size_t avail, DecodedCtx &d)
   return true;
 }
 
+// Upload the per-element block {Cm, Ck, Cw, Cx} of a block operator and the block of its transpose: (A^T)'s pointwise form
+// has every tensor transposed, and the value->curl and curl->value tensors trade places.
+int set_block(b2p_op *op, const std::vector<double> &blk)
+{
+  std::vector<double> blk_t(blk.size());
+  static const int from[4] = {0, 1, 3, 2};
+  for (int e = 0; e < op->ne; e++)
+    for (int k = 0; k < 4; k++)
+      for (int i = 0; i < 3; i++)
+        for (int j = 0; j < 3; j++) blk_t[36 * (size_t)e + 9 * k + i + 3 * j] = blk[36 * (size_t)e + 9 * from[k] + j + 3 * i];
+  if (op->bcoef)  // refill in place: p-coarsened operators share these arrays
+  {
+    B2P_CUDA(op->ctx, cudaMemcpy(op->bcoef, blk.data(), blk.size() * sizeof(double), cudaMemcpyHostToDevice));
+    B2P_CUDA(op->ctx, cudaMemcpy(op->bcoef_t, blk_t.data(), blk_t.size() * sizeof(double), cudaMemcpyHostToDevice));
+    return B2P_SUCCESS;
+  }
+  int rc;
+  if ((rc = upload(op->ctx, blk.data(), blk.size(), &op->bcoef)) || (rc = upload(op->ctx, blk_t.data(), blk_t.size(), &op->bcoef_t)))
+    return rc;
+  return B2P_SUCCESS;
+}
+
 int set_coeff(b2p_op *op, const void *blob, size_t bytes)
 {
   b2p_ctx *ctx = op->ctx;
@@ -435,6 +473,15 @@ int set_coeff(b2p_op *op, const void *blob, size_t bytes)
     for (int part = 0; part < 2; part++)
       for (int t = 0; t < 9; t++) ecoef[18 * (size_t)e + 9 * part + t] = mats[9 * (size_t)emat[2 * (size_t)e + part] + t];
   if ((rc = upload(ctx, ecoef.data(), ecoef.size(), &op->ecoef))) return rc;
+  if (!op->dense && (op->kind == B2P_ND_WEAKCURL || op->kind == B2P_ND_MIXEDCURL))
+  {
+    // the context's tensor goes to Cw (weak curl: values -> curls) or Cx (mixed curl: curls -> values), zeros elsewhere
+    const int slot = op->kind == B2P_ND_WEAKCURL ? 2 : 3;
+    std::vector<double> blk((size_t)36 * op->ne, 0.0);
+    for (int e = 0; e < op->ne; e++)
+      for (int t = 0; t < 9; t++) blk[36 * (size_t)e + 9 * slot + t] = ecoef[18 * (size_t)e + t];
+    return set_block(op, blk);
+  }
   return B2P_SUCCESS;
 }
 
@@ -507,7 +554,9 @@ int assemble_qdata(b2p_op *op)
 int b2p_op_create(b2p_ctx *ctx, b2p_geom *geom, const b2p_op_desc *d, b2p_op **out)
 {
   B2P_CHECK(ctx, ctx && geom && d && out, B2P_ERR_ARG, "b2p_op_create: null argument");
-  B2P_CHECK(ctx, d->kind >= B2P_CURLCURL && d->kind <= B2P_H1_DIFFUSION, B2P_ERR_ARG, "b2p_op_create: bad kind %d", d->kind);
+  B2P_CHECK(ctx, d->kind >= B2P_CURLCURL && d->kind <= B2P_ND_MIXEDCURL, B2P_ERR_ARG, "b2p_op_create: bad kind %d", d->kind);
+  B2P_CHECK(ctx, !(d->assemble_qdata && (d->kind == B2P_ND_WEAKCURL || d->kind == B2P_ND_MIXEDCURL)), B2P_ERR_UNSUPPORTED,
+            "b2p_op_create: assembled q-data is not available for the mixed curl kinds (apply their coefficient on the fly)");
   B2P_CHECK(ctx, d->ne == geom->ne, B2P_ERR_ARG, "b2p_op_create: %d elements vs %d in geometry", d->ne, geom->ne);
   B2P_CHECK(ctx, d->p >= 1 && d->p <= 6 && d->p < geom->q1d && geom->q1d <= 7, B2P_ERR_UNSUPPORTED,
             "b2p_op_create: unsupported p=%d q1d=%d (hex kernels cover p<=6, p<q1d<=7)", d->p, geom->q1d);
@@ -657,6 +706,8 @@ int b2p_op_coarsen(b2p_op *fine, const b2p_op_desc *d, b2p_op **out)
   op->mat = fine->mat;
   op->emat = fine->emat;
   op->ecoef = fine->ecoef;
+  op->bcoef = fine->bcoef;
+  op->bcoef_t = fine->bcoef_t;
   op->iso = fine->iso;
   op->n_mat = fine->n_mat;
   op->aq = fine->aq;
@@ -700,7 +751,7 @@ int b2p_op_apply_add_pair(b2p_op *op, double alpha, const double *x0, const doub
     B2P_CHECK(op->ctx, op->lidx_bc, B2P_ERR_ARG, "b2p_op_apply_add_pair: masked apply without b2p_op_set_essential");
     lidx = op->lidx_bc;
   }
-  if (!nd_hex_apply4z_eligible(op) || !op->ecoef)
+  if (op->bcoef || !nd_hex_apply4z_eligible(op) || !op->ecoef)
   {
     int rc = b2p::apply_range(op, lidx, alpha, x0, y0, ApplyRange(), flags, (cudaStream_t)s);
     return rc ? rc : b2p::apply_range(op, lidx, alpha, x1, y1, ApplyRange(), flags, (cudaStream_t)s);
@@ -815,7 +866,8 @@ int64_t b2p_op_algorithmic_bytes(b2p_op *op)
   if (op->dense)  // + the tables once (L2 resident)
     return 16 * op->lsize + (int64_t)op->ne * (4 * (int64_t)op->PS + 80 * Q + 144) + 8 * (int64_t)op->dense_Rpad * op->dense_Ppad;
   const int64_t per_point = op->assembled ? op->aq_ncomp : 10;
-  return 16 * op->lsize + (int64_t)op->ne * (4 * (int64_t)op->PS + 8 * per_point * Q + (op->assembled ? 0 : 144));  // +144: per-element coefficient block
+  // + per-element coefficient block: 144 bytes (two 3x3 tensors), 288 for block operators (four)
+  return 16 * op->lsize + (int64_t)op->ne * (4 * (int64_t)op->PS + 8 * per_point * Q + (op->assembled ? 0 : (op->bcoef ? 288 : 144)));
 }
 
 // One operator for a real sum  sum_t c_t A_t  of sum-factorised ND operators over the same geometry, space and essential
@@ -828,6 +880,34 @@ static int sum_fill_coefficients(b2p_op *sum, int n_terms, b2p_op *const *ops, c
   b2p_ctx *ctx = sum->ctx;
   const int ne = sum->ne;
   std::vector<double> e18((size_t)18 * ne), z((size_t)18 * ne, 0.0);
+  bool block = false;
+  for (int t = 0; t < n_terms; t++) block = block || ops[t]->bcoef;
+  if (block)
+  {
+    // a mixed curl term makes the sum a block operator: each term's tensors go to their slots of {Cm, Ck, Cw, Cx}
+    std::vector<double> b36((size_t)36 * ne), z36((size_t)36 * ne, 0.0);
+    for (int t = 0; t < n_terms; t++)
+    {
+      const b2p_op *o = ops[t];
+      if (o->bcoef)
+      {
+        B2P_CUDA(ctx, cudaMemcpy(b36.data(), o->bcoef, b36.size() * sizeof(double), cudaMemcpyDeviceToHost));
+        for (size_t i = 0; i < z36.size(); i++) z36[i] += coefs[t] * b36[i];
+        continue;
+      }
+      B2P_CUDA(ctx, cudaMemcpy(e18.data(), o->ecoef, e18.size() * sizeof(double), cudaMemcpyDeviceToHost));
+      const bool m = (o->kind == B2P_ND_MASS || o->kind == B2P_CURLCURL_MASS), k = (o->kind == B2P_CURLCURL || o->kind == B2P_CURLCURL_MASS);
+      for (int e = 0; e < ne; e++)
+        for (int i = 0; i < 9; i++)
+        {
+          if (m) z36[(size_t)36 * e + i] += coefs[t] * e18[(size_t)18 * e + i];
+          if (k) z36[(size_t)36 * e + 9 + i] += coefs[t] * e18[(size_t)18 * e + 9 + i];
+        }
+    }
+    sum->kind = B2P_ND_BLOCK;
+    sum->iso = false;
+    return set_block(sum, z36);
+  }
   bool mass = false, curl = false;
   for (int t = 0; t < n_terms; t++)
   {
@@ -888,8 +968,9 @@ int b2p_op_create_sum(b2p_ctx *ctx, int n_terms, b2p_op *const *ops, const doubl
   for (int t = 0; t < n_terms; t++)
   {
     const b2p_op *o = ops[t];
-    B2P_CHECK(ctx, o && o->dense == dense && !o->assembled && o->kind >= B2P_CURLCURL && o->kind <= B2P_CURLCURL_MASS && o->ecoef,
-              B2P_ERR_UNSUPPORTED, "b2p_op_create_sum: term %d is not an ND curl-curl / mass operator with on-the-fly coefficients", t);
+    // sum-factorised block operators (mixed curl kinds) fuse too; dense mixed terms do not
+    B2P_CHECK(ctx, o && o->dense == dense && !o->assembled && ((o->kind >= B2P_CURLCURL && o->kind <= B2P_CURLCURL_MASS && o->ecoef) || o->bcoef),
+              B2P_ERR_UNSUPPORTED, "b2p_op_create_sum: term %d is not an ND curl-curl / mass / mixed curl operator with on-the-fly coefficients", t);
     B2P_CHECK(ctx, o->geom == o0->geom && o->p == o0->p && o->q1d == o0->q1d && o->ne == o0->ne && o->lsize == o0->lsize && o->PS == o0->PS &&
                        o->P == o0->P && o->dense_Ppad == o0->dense_Ppad && (o->curl_orient != nullptr) == (o0->curl_orient != nullptr) &&
                        (o->lidx_bc != nullptr) == (o0->lidx_bc != nullptr),
@@ -1020,6 +1101,8 @@ void b2p_op_destroy(b2p_op *op)
     cudaFree(op->mat);
     cudaFree(op->emat);
     cudaFree(op->ecoef);
+    cudaFree(op->bcoef);
+    cudaFree(op->bcoef_t);
     cudaFree(op->aq);
   }
   b2p_geom_destroy(op->geom);

@@ -1,4 +1,5 @@
-// Matrix-free Nedelec (H(curl)) hexahedron operators: curl-curl, mass, curl-curl + mass.
+// Matrix-free Nedelec (H(curl)) hexahedron operators: curl-curl, mass, curl-curl + mass, and the block form of the mixed
+// curl kinds and their sums (B2P_ND_BLOCK: value and curl at every point, coupled by four 3x3 tensors per element).
 //
 //   y_L += sum_e E_e^T  B^T  D  B  E_e x_L
 //
@@ -53,16 +54,19 @@ struct NDParams
   int ne;
   int PS;  // padded restriction row stride
   VSplit sp;
+  const double *bcoef;  // B2P_ND_BLOCK: [ne][36] {Cm, Ck, Cw, Cx} (the transposed block for a transposed apply)
 };
 
-// KIND: B2P_CURLCURL / B2P_ND_MASS / B2P_CURLCURL_MASS. ASM: assembled q-data.
+// KIND: B2P_CURLCURL / B2P_ND_MASS / B2P_CURLCURL_MASS / B2P_ND_BLOCK. ASM: assembled q-data.
 template <int P_, int Q_, int KIND, bool ASM, int NEB, int NT>
 __global__ void __launch_bounds__(NT) nd_hex_apply_kernel(NDParams prm)
 {
   using L = NDLayout<P_, Q_>;
   constexpr int p = L::p, q = L::q, n = L::n, P = L::P, Q = L::Q, D3 = L::D3, N1 = L::N1, N2 = L::N2;
-  constexpr bool MASS = (KIND == B2P_ND_MASS || KIND == B2P_CURLCURL_MASS);
-  constexpr bool CURL = (KIND == B2P_CURLCURL || KIND == B2P_CURLCURL_MASS);
+  constexpr bool BLOCK = (KIND == B2P_ND_BLOCK);
+  constexpr bool MASS = (KIND == B2P_ND_MASS || KIND == B2P_CURLCURL_MASS || BLOCK);
+  constexpr bool CURL = (KIND == B2P_CURLCURL || KIND == B2P_CURLCURL_MASS || BLOCK);
+  static_assert(!(BLOCK && ASM), "block operators have no assembled q-data");
   constexpr int ES = L::PER_ELEM;
 
   B2P_DYN_SMEM(double, smem);
@@ -169,6 +173,40 @@ __global__ void __launch_bounds__(NT) nd_hex_apply_kernel(NDParams prm)
         cqe[2 * Q + iq] = a[2 * Q] * u0 + a[5 * Q] * u1 + a[8 * Q] * u2;
       }
     }
+    else if (BLOCK)
+    {
+      const double *g = prm.qd + (size_t)(e0 + e) * 10 * Q + sq;
+      const double *C = prm.bcoef + 36 * (size_t)(e0 + e);
+      double A[9], Jd[9], Cm[9], Ck[9], Cw[9], Cx[9];
+#pragma unroll
+      for (int i = 0; i < 9; i++)
+      {
+        A[i] = g[(1 + i) * Q];
+        Cm[i] = __ldg(C + i);
+        Ck[i] = __ldg(C + 9 + i);
+        Cw[i] = __ldg(C + 18 + i);
+        Cx[i] = __ldg(C + 27 + i);
+      }
+      cofactor33(A, Jd);
+      const double u[3] = {uqe[iq], uqe[Q + iq], uqe[2 * Q + iq]}, c[3] = {cqe[iq], cqe[Q + iq], cqe[2 * Q + iq]};
+      double t[3], s[3], a[3], b[3], zv[3], zc[3], v[3], w[3];
+      Ax33(A, u, t);
+      Ax33(Jd, c, s);
+      Ax33(Cm, t, a);
+      Ax33(Cx, s, b);
+      for (int i = 0; i < 3; i++) zv[i] = a[i] + b[i];
+      Ax33(Ck, s, a);
+      Ax33(Cw, t, b);
+      for (int i = 0; i < 3; i++) zc[i] = a[i] + b[i];
+      Atx33(A, zv, g[0], v);
+      Atx33(Jd, zc, g[0], w);
+      uqe[iq] = v[0];
+      uqe[Q + iq] = v[1];
+      uqe[2 * Q + iq] = v[2];
+      cqe[iq] = w[0];
+      cqe[Q + iq] = w[1];
+      cqe[2 * Q + iq] = w[2];
+    }
     else
     {
       const double *g = prm.qd + (size_t)(e0 + e) * 10 * Q + sq;
@@ -272,6 +310,7 @@ template <int KIND>
 __global__ void nd_hex_diag_kernel(NDParams prm, int p, int q, bool assembled)
 {
   const int n = p + 1, P = 3 * p * n * n, Q = q * q * q, D3 = p * n * n;
+  constexpr bool BLOCK = (KIND == B2P_ND_BLOCK);
   constexpr bool MASS = (KIND == B2P_ND_MASS || KIND == B2P_CURLCURL_MASS);
   constexpr bool CURL = (KIND == B2P_CURLCURL || KIND == B2P_CURLCURL_MASS);
   const double *Bo = prm.tab, *Bc = Bo + q * p, *Gc = Bc + q * n;
@@ -285,7 +324,7 @@ __global__ void nd_hex_diag_kernel(NDParams prm, int p, int q, bool assembled)
   else { i = r % n; j = (r / n) % n; k = r / (n * n); }
   double C0[9], C1[9];
   const int32_t *em = prm.emat + 2 * (size_t)e;
-  if (!assembled)
+  if (!assembled && !BLOCK)
   {
     for (int t = 0; t < 9; t++)
     {
@@ -312,7 +351,27 @@ __global__ void nd_hex_diag_kernel(NDParams prm, int p, int q, bool assembled)
         if (c == 0) { cu[1] = fx * fy * gz; cu[2] = -fx * gy * fz; }
         else if (c == 1) { cu[0] = -fx * fy * gz; cu[2] = gx * fy * fz; }
         else { cu[0] = fx * gy * fz; cu[1] = -gx * fy * fz; }
-        if (assembled)
+        if (BLOCK)
+        {
+          // u^T (w A^T (Cm A u + Cx Jd cu)) + cu^T (w Jd^T (Ck Jd cu + Cw A u))
+          const double *g = prm.qd + (size_t)e * 10 * Q + iq, *C = prm.bcoef + 36 * (size_t)e;
+          double A[9], Jd[9], t[3], sc[3], a[3], b[3], z[3], v[3];
+          for (int tt = 0; tt < 9; tt++) A[tt] = g[(1 + tt) * Q];
+          cofactor33(A, Jd);
+          Ax33(A, u, t);
+          Ax33(Jd, cu, sc);
+          Ax33(C, t, a);
+          Ax33(C + 27, sc, b);
+          for (int d = 0; d < 3; d++) z[d] = a[d] + b[d];
+          Atx33(A, z, g[0], v);
+          s += u[0] * v[0] + u[1] * v[1] + u[2] * v[2];
+          Ax33(C + 9, sc, a);
+          Ax33(C + 18, t, b);
+          for (int d = 0; d < 3; d++) z[d] = a[d] + b[d];
+          Atx33(Jd, z, g[0], v);
+          s += cu[0] * v[0] + cu[1] * v[1] + cu[2] * v[2];
+        }
+        else if (assembled)
         {
           const double *a = prm.aq + (size_t)e * prm.aq_estride + iq;
           if (MASS)
@@ -382,9 +441,12 @@ __global__ void nd_assemble_qdata_kernel(NDParams prm, int Q, double *aq)
   }
 }
 
-NDParams make_params(b2p_op *op, const int32_t *lidx, double alpha, const double *x, double *y, const ApplyRange &rg = ApplyRange())
+NDParams make_params(b2p_op *op, const int32_t *lidx, double alpha, const double *x, double *y, const ApplyRange &rg = ApplyRange(),
+                     bool transpose = false)
 {
   NDParams prm;
+  const double *bc = transpose ? op->bcoef_t : op->bcoef;
+  prm.bcoef = bc ? bc + 36 * (size_t)rg.e_off : nullptr;
   const int e_off = rg.e_off, e_cnt = rg.e_cnt < 0 ? op->ne - rg.e_off : rg.e_cnt;
   prm.lidx = lidx + (size_t)e_off * op->PS;
   prm.alpha = alpha;
@@ -405,7 +467,8 @@ NDParams make_params(b2p_op *op, const int32_t *lidx, double alpha, const double
 }
 
 template <int P_, int Q_, int KIND, bool ASM>
-int launch_pq(b2p_op *op, const int32_t *lidx, double alpha, const double *x, double *y, const ApplyRange &rg, cudaStream_t s)
+int launch_pq(b2p_op *op, const int32_t *lidx, double alpha, const double *x, double *y, const ApplyRange &rg, cudaStream_t s,
+              bool transpose = false)
 {
   using L = NDLayout<P_, Q_>;
   // elements per block: keep shared memory under ~96 KB and at least 128 threads of work
@@ -424,15 +487,17 @@ int launch_pq(b2p_op *op, const int32_t *lidx, double alpha, const double *x, do
   const int ne_run = rg.e_cnt < 0 ? op->ne - rg.e_off : rg.e_cnt;
   if (ne_run <= 0) return B2P_SUCCESS;
   const int grid = (ne_run + NEB - 1) / NEB;
-  B2P_LAUNCH(kern, grid, NT, shmem, s, make_params(op, lidx, alpha, x, y, rg));
+  B2P_LAUNCH(kern, grid, NT, shmem, s, make_params(op, lidx, alpha, x, y, rg, transpose));
   B2P_CUDA(op->ctx, cudaGetLastError());
   return B2P_SUCCESS;
 }
 
 template <int P_, int Q_>
-int launch_kind(b2p_op *op, const int32_t *lidx, double alpha, const double *x, double *y, const ApplyRange &rg, cudaStream_t s)
+int launch_kind(b2p_op *op, const int32_t *lidx, double alpha, const double *x, double *y, const ApplyRange &rg, cudaStream_t s,
+                bool transpose)
 {
   const bool a = op->assembled;
+  if (op->bcoef) return launch_pq<P_, Q_, B2P_ND_BLOCK, false>(op, lidx, alpha, x, y, rg, s, transpose);
   switch (op->kind)
   {
     case B2P_CURLCURL:
@@ -449,10 +514,11 @@ int launch_kind(b2p_op *op, const int32_t *lidx, double alpha, const double *x, 
 
 }  // namespace
 
-int launch_nd_hex_apply(b2p_op *op, const int32_t *lidx, double alpha, const double *x, double *y, const ApplyRange &rg, cudaStream_t s)
+int launch_nd_hex_apply(b2p_op *op, const int32_t *lidx, double alpha, const double *x, double *y, const ApplyRange &rg, cudaStream_t s,
+                        bool transpose)
 {
 #define B2P_CASE(PP, QQ) \
-  if (op->p == PP && op->q1d == QQ) return launch_kind<PP, QQ>(op, lidx, alpha, x, y, rg, s);
+  if (op->p == PP && op->q1d == QQ) return launch_kind<PP, QQ>(op, lidx, alpha, x, y, rg, s, transpose);
   // (p, q1d): q1d = p+1 for a stand-alone operator; larger q1d for p-coarsened operators that
   // reuse the fine level's quadrature (CeedOperatorCoarsen, libceed/operator.cpp:525-585).
   B2P_CASE(1, 2) B2P_CASE(1, 3) B2P_CASE(1, 4) B2P_CASE(1, 5) B2P_CASE(1, 6) B2P_CASE(1, 7)
@@ -472,6 +538,12 @@ int launch_nd_hex_diag(b2p_op *op, double *diag, cudaStream_t s)
   const size_t total = (size_t)op->ne * op->P;
   const int nt = 128;
   const unsigned grid = (unsigned)((total + nt - 1) / nt);
+  if (op->bcoef)
+  {
+    B2P_LAUNCH(nd_hex_diag_kernel<B2P_ND_BLOCK>, grid, nt, 0, s, prm, op->p, op->q1d, false);
+    B2P_CUDA(op->ctx, cudaGetLastError());
+    return B2P_SUCCESS;
+  }
   switch (op->kind)
   {
     case B2P_CURLCURL: B2P_LAUNCH(nd_hex_diag_kernel<B2P_CURLCURL>, grid, nt, 0, s, prm, op->p, op->q1d, op->assembled); break;

@@ -97,10 +97,12 @@ struct ND6Layout
 {
   static constexpr int p = P_, q = Q_, n = P_ + 1, Q = q * q * q, P = 3 * p * n * n, D3 = p * n * n;
   static constexpr int PS = (P + 3) & ~3;
-  static constexpr bool MASS = (KIND == B2P_ND_MASS || KIND == B2P_CURLCURL_MASS);
-  static constexpr bool CURL = (KIND == B2P_CURLCURL || KIND == B2P_CURLCURL_MASS);
+  // B2P_ND_BLOCK: the CURLCURL_MASS data flow (and its row pads) with the four-tensor block of b2p_op::bcoef in the D phase
+  static constexpr bool BLOCK = (KIND == B2P_ND_BLOCK);
+  static constexpr bool MASS = (KIND == B2P_ND_MASS || KIND == B2P_CURLCURL_MASS || BLOCK);
+  static constexpr bool CURL = (KIND == B2P_CURLCURL || KIND == B2P_CURLCURL_MASS || BLOCK);
   static constexpr int NEW = (q * q >= 32) ? 1 : 32 / (q * q);
-  static constexpr Nd6Pad PAD = nd6_pads(P_, Q_, KIND);
+  static constexpr Nd6Pad PAD = nd6_pads(P_, Q_, BLOCK ? B2P_CURLCURL_MASS : KIND);
   static constexpr int NXA = p * q, NNA = n * q;
   static constexpr int A_XA = 0, A_XB = A_XA + NEW * NXA, A_ZA = A_XB + (CURL ? NEW * NXA : 0), LA = A_ZA + NEW * NNA,
                        RSA = LA + PAD.a;
@@ -112,7 +114,7 @@ struct ND6Layout
   static constexpr int Y0 = ALIAS ? 0 : ZSZ, WEND = (ALIAS && ZSZ > q * RSY) ? ZSZ : Y0 + q * RSY, WTOT = (WEND + 1) & ~1;
   static constexpr int LSX = nd6_lane_stride(p * n, NEW), LSZ = nd6_lane_stride(n * n, NEW);
   static constexpr int GE = 10 * Q;   // doubles of q-data per element
-  static constexpr int CE = 18;       // coefficient matrices per element
+  static constexpr int CE = BLOCK ? 36 : 18;  // coefficient doubles per element: two 3x3 tensors, four for the block form
   // one ring slot: the batch's index rows followed by its coefficient blocks (one mbarrier, one transaction count)
   static constexpr int SLOT_I = NEW * PS * 4, SLOT_C = NEW * CE * 8, SLOT = (SLOT_I + SLOT_C + 15) & ~15;
   static constexpr int OFF_G = 0;                     // [NEW * GE] doubles of staged q-data (GSM)
@@ -635,7 +637,25 @@ __global__ void __launch_bounds__(NW * 32, MINB) nd_hex_apply6_kernel(const __gr
         double v[3] = {0, 0, 0}, cw[3] = {0, 0, 0};
         const double wdetJ = ok ? alpha * gq[0] : 0.0;  // alpha folded into the quadrature weight; tail slots contribute zero
         const double *A = gq + 1;
-        if (prm.iso)
+        if constexpr (L::BLOCK)
+        {
+          // out_val = w A^T (Cm A u + Cx Jd c),  out_curl = w Jd^T (Ck Jd c + Cw A u)
+          double Jd[9], t[3], sc[3], a[3], b[3], z[3];
+          cofactor33(A, Jd);
+          Ax33(A, uu[qx], t);
+          Ax33(Jd, cc[qx], sc);
+          Ax33(C, t, a);
+          Ax33(C + 27, sc, b);
+#pragma unroll
+          for (int r = 0; r < 3; r++) z[r] = a[r] + b[r];
+          Atx33(A, z, wdetJ, v);
+          Ax33(C + 9, sc, a);
+          Ax33(C + 18, t, b);
+#pragma unroll
+          for (int r = 0; r < 3; r++) z[r] = a[r] + b[r];
+          Atx33(Jd, z, wdetJ, cw);
+        }
+        else if (prm.iso)
         {
           if (MASS) AtAx(A, uu[qx], wdetJ * C[0], v);
           if (CURL)
@@ -880,7 +900,8 @@ __global__ void __launch_bounds__(NW * 32, MINB) nd_hex_apply6_kernel(const __gr
 }
 
 template <int P_, int Q_, int KIND, int NW, int MINB, bool FWD, bool GSM, bool XLATE, bool WITH_SPLIT, bool GL1 = false>
-int launch6_cfg(b2p_op *op, const int32_t *lidx, double alpha, const double *x, double *y, const ApplyRange &rg, cudaStream_t s)
+int launch6_cfg(b2p_op *op, const int32_t *lidx, double alpha, const double *x, double *y, const ApplyRange &rg, cudaStream_t s,
+                bool transpose = false)
 {
   using L = ND6Layout<P_, Q_, KIND, FWD, GSM>;
   const size_t shmem = (size_t)NW * L::WS;
@@ -910,7 +931,10 @@ int launch6_cfg(b2p_op *op, const int32_t *lidx, double alpha, const double *x, 
   if (e_cnt <= 0) return B2P_SUCCESS;
   prm.lidx = lidx + (size_t)e_off * op->PS;
   prm.qd = op->geom->qd + (size_t)e_off * 10 * op->geom->Q;
-  prm.ecoef = op->ecoef + 18 * (size_t)e_off;
+  if constexpr (L::BLOCK)
+    prm.ecoef = (transpose ? op->bcoef_t : op->bcoef) + L::CE * (size_t)e_off;
+  else
+    prm.ecoef = op->ecoef + L::CE * (size_t)e_off;
   prm.x = x;
   prm.y = y;
   prm.sink = op->ctx->d_sink;
@@ -923,7 +947,7 @@ int launch6_cfg(b2p_op *op, const int32_t *lidx, double alpha, const double *x, 
   prm.wait_expect = rg.wait_expect;
   prm.wait_n = rg.wait_n;
   prm.wait_from_elem = rg.wait_from_elem;
-  prm.iso = op->iso ? 1 : 0;
+  prm.iso = (op->iso && !L::BLOCK) ? 1 : 0;
   const int n = P_ + 1;
   constexpr int H = ND6Params<P_, Q_>::H;
   for (int i = 0; i < H * P_; i++) prm.Bo[i] = op->h_tab[i];
@@ -958,7 +982,8 @@ constexpr int ND6_NW = 4, ND6_MINB = 2;
 constexpr bool ND6_FWD = true, ND6_GSM = true, ND6_XLATE = true;
 
 template <int P_, int Q_, int KIND>
-int launch6(b2p_op *op, const int32_t *lidx, double alpha, const double *x, double *y, const ApplyRange &rg, cudaStream_t s)
+int launch6(b2p_op *op, const int32_t *lidx, double alpha, const double *x, double *y, const ApplyRange &rg, cudaStream_t s,
+            bool transpose = false)
 {
 #ifdef B2P_ND6_EXPERIMENTS
   if constexpr (P_ == 3 && KIND == B2P_CURLCURL_MASS)
@@ -984,7 +1009,7 @@ int launch6(b2p_op *op, const int32_t *lidx, double alpha, const double *x, doub
     }
   }
 #endif
-  return launch6_cfg<P_, Q_, KIND, ND6_NW, ND6_MINB, ND6_FWD, ND6_GSM, ND6_XLATE, true>(op, lidx, alpha, x, y, rg, s);
+  return launch6_cfg<P_, Q_, KIND, ND6_NW, ND6_MINB, ND6_FWD, ND6_GSM, ND6_XLATE, true>(op, lidx, alpha, x, y, rg, s, transpose);
 }
 
 }  // namespace
@@ -1012,17 +1037,19 @@ bool nd_tables_symmetric(const double *tab, int p, int q, double rel_tol)
 
 bool nd_hex_apply6_eligible(b2p_op *op)
 {
-  if (!op || op->dense || op->assembled || op->kind == B2P_H1_DIFFUSION || !op->ecoef) return false;
+  if (!op || op->dense || op->assembled || op->kind == B2P_H1_DIFFUSION || !(op->ecoef || op->bcoef)) return false;
   if (!(op->q1d == op->p + 1 && op->p >= 2 && op->p <= 3)) return false;
   if (op->tab_sym6 < 0) op->tab_sym6 = nd_tables_symmetric(op->h_tab.data(), op->p, op->q1d, 4e-16) ? 1 : 0;
   return op->tab_sym6 == 1;
 }
 
-int launch_nd_hex_apply6(b2p_op *op, const int32_t *lidx, double alpha, const double *x, double *y, const ApplyRange &rg, cudaStream_t s)
+int launch_nd_hex_apply6(b2p_op *op, const int32_t *lidx, double alpha, const double *x, double *y, const ApplyRange &rg, cudaStream_t s,
+                         bool transpose)
 {
 #define B2P_CASE(PP, QQ)                                                                                                  \
   if (op->p == PP && op->q1d == QQ)                                                                                       \
   {                                                                                                                       \
+    if (op->bcoef) return launch6<PP, QQ, B2P_ND_BLOCK>(op, lidx, alpha, x, y, rg, s, transpose);                        \
     switch (op->kind)                                                                                                     \
     {                                                                                                                     \
       case B2P_CURLCURL: return launch6<PP, QQ, B2P_CURLCURL>(op, lidx, alpha, x, y, rg, s);                              \

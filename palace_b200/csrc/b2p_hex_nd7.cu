@@ -73,8 +73,11 @@ struct ND7Layout
 {
   static constexpr int p = P_, q = P_ + 1, n = P_ + 1, QQ = q * q, Q = q * q * q, D3 = p * n * n, P = 3 * D3;
   static constexpr int PS = (P + 3) & ~3;
-  static constexpr bool MASS = (KIND == B2P_ND_MASS || KIND == B2P_CURLCURL_MASS);
-  static constexpr bool CURL = (KIND == B2P_CURLCURL || KIND == B2P_CURLCURL_MASS);
+  // B2P_ND_BLOCK: the CURLCURL_MASS data flow with the four-tensor block of b2p_op::bcoef in the D phase
+  static constexpr bool BLOCK = (KIND == B2P_ND_BLOCK);
+  static constexpr bool MASS = (KIND == B2P_ND_MASS || KIND == B2P_CURLCURL_MASS || BLOCK);
+  static constexpr bool CURL = (KIND == B2P_CURLCURL || KIND == B2P_CURLCURL_MASS || BLOCK);
+  static constexpr int CE = BLOCK ? 36 : 18;  // coefficient doubles per element: two 3x3 tensors, four for the block form
   static constexpr int LQ = NE * QQ;  // line slots of one component (all index extents padded to q)
   // Z -> Y arrays (region A), rows j: written by the Z phase at (j, i + q qz), read by the Y phase along j
   static constexpr int RS1 = nd7_stride(LQ, q);
@@ -88,8 +91,8 @@ struct ND7Layout
   static constexpr int B_X1 = 0, B_X2 = B_X1 + (MASS ? p * RS2 : 0), B_X3 = B_X2 + (CURL ? p * RS2 : 0),
                        B_Y1 = B_X3 + (CURL ? p * RS2 : 0), B_Y2 = B_Y1 + n * RS2, B_Z1 = B_Y2 + (CURL ? n * RS2 : 0),
                        B_Z3 = B_Z1 + n * RS2, SB = B_Z3 + (CURL ? n * RS2 : 0);
-  // GSM: q-data [NE][10][Q] and coefficient blocks [NE][18] of the batch, staged by TMA bulk copies behind one mbarrier
-  static constexpr int GE = 10 * Q, OFF_G = (SA + SB + 1) & ~1, OFF_C = OFF_G + NE * GE, OFF_BAR = OFF_C + NE * 18;
+  // GSM: q-data [NE][10][Q] and coefficient blocks [NE][CE] of the batch, staged by TMA bulk copies behind one mbarrier
+  static constexpr int GE = 10 * Q, OFF_G = (SA + SB + 1) & ~1, OFF_C = OFF_G + NE * GE, OFF_BAR = OFF_C + NE * CE;
   static_assert(GE % 2 == 0, "16-byte blocks for the bulk copies");
   static constexpr int SMEM_BYTES_LDG = (SA + SB) * 8, SMEM_BYTES_GSM = (OFF_BAR + 2) * 8;
 };
@@ -217,9 +220,9 @@ __global__ void __launch_bounds__(3 * WPC * 32, MINB) nd_hex_apply7_kernel(const
   auto issue_geom = [&](int bb)  // (one thread)
   {
     const int e0 = bb * NE, nel = min(NE, prm.ne - e0);
-    mbar_expect_tx(bar_g, (uint32_t)(nel * (L::GE + 18) * sizeof(double)));
+    mbar_expect_tx(bar_g, (uint32_t)(nel * (L::GE + L::CE) * sizeof(double)));
     tma_bulk_g2s(sG, prm.qd + (size_t)e0 * L::GE, (uint32_t)(nel * L::GE * sizeof(double)), bar_g);
-    tma_bulk_g2s(sC, prm.ecoef + (size_t)e0 * 18, (uint32_t)(nel * 18 * sizeof(double)), bar_g);
+    tma_bulk_g2s(sC, prm.ecoef + (size_t)e0 * L::CE, (uint32_t)(nel * L::CE * sizeof(double)), bar_g);
   };
   uint32_t par_g = 0;
   if (GSM)
@@ -460,7 +463,7 @@ __global__ void __launch_bounds__(3 * WPC * 32, MINB) nd_hex_apply7_kernel(const
       const int qx = iota / LQ, t = iota % LQ, e = t / QQ, rr = t % QQ;
       if (e >= nel) continue;  // (tail slots hold zeros)
       const double *g = GSM ? sG + e * L::GE + qx * QQ + rr : prm.qd + (size_t)(e0 + e) * L::GE + qx * QQ + rr;
-      const double *C = GSM ? sC + e * 18 : prm.ecoef + (size_t)(e0 + e) * 18;
+      const double *C = GSM ? sC + e * L::CE : prm.ecoef + (size_t)(e0 + e) * L::CE;
       double A[9], Cm[9], wdetJ, cm0, cc0;
       if (GSM)
       {
@@ -486,7 +489,33 @@ __global__ void __launch_bounds__(3 * WPC * 32, MINB) nd_hex_apply7_kernel(const
         if (MASS) u[r3] = pu[r3 * NE * Q];
         if (CURL) c[r3] = pc[r3 * NE * Q];
       }
-      if (prm.iso)
+      if constexpr (L::BLOCK)
+      {
+        // out_val = w A^T (Cm A u + Cx Jd c),  out_curl = w Jd^T (Ck Jd c + Cw A u)
+        double Jd[9], Ck[9], Cw[9], Cx[9], t[3], sc[3], a[3], b[3], z[3];
+#pragma unroll
+        for (int i = 0; i < 9; i++)
+        {
+          Cm[i] = GSM ? C[i] : __ldg(C + i);
+          Ck[i] = GSM ? C[9 + i] : __ldg(C + 9 + i);
+          Cw[i] = GSM ? C[18 + i] : __ldg(C + 18 + i);
+          Cx[i] = GSM ? C[27 + i] : __ldg(C + 27 + i);
+        }
+        cofactor33(A, Jd);
+        Ax33(A, u, t);
+        Ax33(Jd, c, sc);
+        Ax33(Cm, t, a);
+        Ax33(Cx, sc, b);
+#pragma unroll
+        for (int r = 0; r < 3; r++) z[r] = a[r] + b[r];
+        Atx33(A, z, wdetJ, v);
+        Ax33(Ck, sc, a);
+        Ax33(Cw, t, b);
+#pragma unroll
+        for (int r = 0; r < 3; r++) z[r] = a[r] + b[r];
+        Atx33(Jd, z, wdetJ, cw);
+      }
+      else if (prm.iso)
       {
         if (MASS) AtAx(A, u, wdetJ * cm0, v);
         if (CURL)
@@ -749,7 +778,8 @@ struct ND7Shape<6>
 };
 
 template <int P_, int KIND, int NE, int WPC, int MINB, bool GSM, bool CBAR>
-int launch7_cfg(b2p_op *op, const int32_t *lidx, double alpha, const double *x, double *y, const ApplyRange &rg, cudaStream_t s)
+int launch7_cfg(b2p_op *op, const int32_t *lidx, double alpha, const double *x, double *y, const ApplyRange &rg, cudaStream_t s,
+                bool transpose = false)
 {
   using L = ND7Layout<P_, KIND, NE>;
   constexpr int NT = 3 * WPC * 32;
@@ -767,7 +797,10 @@ int launch7_cfg(b2p_op *op, const int32_t *lidx, double alpha, const double *x, 
   if (e_cnt <= 0) return B2P_SUCCESS;
   prm.lidx = lidx + (size_t)e_off * op->PS;
   prm.qd = op->geom->qd + (size_t)e_off * 10 * op->geom->Q;
-  prm.ecoef = op->ecoef + 18 * (size_t)e_off;
+  if constexpr (L::BLOCK)
+    prm.ecoef = (transpose ? op->bcoef_t : op->bcoef) + L::CE * (size_t)e_off;
+  else
+    prm.ecoef = op->ecoef + L::CE * (size_t)e_off;
   prm.x = x;
   prm.y = y;
   prm.sink = op->ctx->d_sink;
@@ -780,7 +813,7 @@ int launch7_cfg(b2p_op *op, const int32_t *lidx, double alpha, const double *x, 
   prm.wait_expect = rg.wait_expect;
   prm.wait_n = rg.wait_n;
   prm.wait_from_elem = rg.wait_from_elem;
-  prm.iso = op->iso ? 1 : 0;
+  prm.iso = (op->iso && !L::BLOCK) ? 1 : 0;
   constexpr int q = P_ + 1, n = P_ + 1;
   for (int i = 0; i < q * P_; i++) prm.Bo[i] = op->h_tab[i];
   for (int i = 0; i < q * n; i++) prm.Bc[i] = op->h_tab[q * P_ + i];
@@ -808,7 +841,8 @@ inline int nd7_cfg_code()
 }
 
 template <int P_, int KIND>
-int launch7(b2p_op *op, const int32_t *lidx, double alpha, const double *x, double *y, const ApplyRange &rg, cudaStream_t s)
+int launch7(b2p_op *op, const int32_t *lidx, double alpha, const double *x, double *y, const ApplyRange &rg, cudaStream_t s,
+            bool transpose = false)
 {
   using S = ND7Shape<P_>;
   if constexpr (KIND == B2P_CURLCURL_MASS)
@@ -834,14 +868,14 @@ int launch7(b2p_op *op, const int32_t *lidx, double alpha, const double *x, doub
     }
 #undef B2P_CFG
   }
-  return launch7_cfg<P_, KIND, S::NE, S::WPC, S::MINB, S::GSM, S::CBAR>(op, lidx, alpha, x, y, rg, s);
+  return launch7_cfg<P_, KIND, S::NE, S::WPC, S::MINB, S::GSM, S::CBAR>(op, lidx, alpha, x, y, rg, s, transpose);
 }
 
 }  // namespace
 
 bool nd_hex_apply7_eligible(b2p_op *op)
 {
-  if (!op || op->dense || op->assembled || op->kind == B2P_H1_DIFFUSION || !op->ecoef) return false;
+  if (!op || op->dense || op->assembled || op->kind == B2P_H1_DIFFUSION || !(op->ecoef || op->bcoef)) return false;
   if (!(op->q1d == op->p + 1 && op->p >= 4 && op->p <= 6)) return false;
   // The kernel reads mirrored table entries through one stored value. Tables evaluated in floating point (MFEM's, or
   // tests/hexspace.py) mirror to a few ulp of the LARGEST entry (measured 6e-16 ... 9e-16 at p = 4, 5): the substitution
@@ -850,11 +884,13 @@ bool nd_hex_apply7_eligible(b2p_op *op)
   return op->tab_sym7 == 1;
 }
 
-int launch_nd_hex_apply7(b2p_op *op, const int32_t *lidx, double alpha, const double *x, double *y, const ApplyRange &rg, cudaStream_t s)
+int launch_nd_hex_apply7(b2p_op *op, const int32_t *lidx, double alpha, const double *x, double *y, const ApplyRange &rg, cudaStream_t s,
+                         bool transpose)
 {
 #define B2P_CASE(PP)                                                                                                  \
   if (op->p == PP && op->q1d == PP + 1)                                                                               \
   {                                                                                                                   \
+    if (op->bcoef) return launch7<PP, B2P_ND_BLOCK>(op, lidx, alpha, x, y, rg, s, transpose);                        \
     switch (op->kind)                                                                                                 \
     {                                                                                                                 \
       case B2P_CURLCURL: return launch7<PP, B2P_CURLCURL>(op, lidx, alpha, x, y, rg, s);                              \

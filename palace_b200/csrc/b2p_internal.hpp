@@ -150,6 +150,11 @@ struct b2p_op
   double *dense_T = nullptr;   // [Rpad][Ppad] stacked interp/deriv tables, zero padded
   int dense_Ppad = 0, dense_Rpad = 0, dense_row_u = -1, dense_row_c = -1;
   int8_t *curl_orient = nullptr;  // [ne][P][3] tridiagonal orientation (ND tets/prisms p >= 2) or null
+  // block operators (the mixed kinds B2P_ND_WEAKCURL / B2P_ND_MIXEDCURL on hexes, and sums that contain one): per element the
+  // four 3x3 tensors {Cm value->value, Ck curl->curl, Cw value->curl, Cx curl->value}, column-major, and the same block for
+  // the transposed operator (every tensor transposed, Cw and Cx swapped). Null for every other operator.
+  double *bcoef = nullptr;     // [ne][36]
+  double *bcoef_t = nullptr;   // [ne][36]
   double *pair_zcoef = nullptr;  // [ne][36] {mass, 0, curl, 0}: coefficient block of the two-vector apply (built on first use)
   int coeff_version = 0, pair_version = -1;  // b2p_op_set_coeff bumps coeff_version (coarsened operators follow their parent's)
   bool owns_coeff = true;  // coarsened operators share the fine operator's coefficient arrays
@@ -192,15 +197,26 @@ struct ApplyRange
   int wait_n = 0, wait_from_elem = 0;
   bool pdl = false;  // launch with programmatic stream serialisation (kernels that call griddep_wait() only)
 };
+// Internal kind of the sum-factorised ND kernels: the pointwise block form of b2p_op::bcoef,
+//   out_val = w detJ A^T (Cm A u + Cx Jd c),   out_curl = w detJ Jd^T (Ck Jd c + Cw A u)   (A = J^-T, Jd = J / detJ).
+constexpr int B2P_ND_BLOCK = 16;
+// Operators that need B2P_APPLY_TRANSPOSE for their transpose (the mixed kinds and block sums).
+inline bool op_nonsymmetric(const b2p_op *op)
+{
+  return op->kind == B2P_ND_WEAKCURL || op->kind == B2P_ND_MIXEDCURL || op->bcoef != nullptr;
+}
 // Kernel launchers (defined in the .cu files).
-int launch_nd_hex_apply(b2p_op *op, const int32_t *lidx, double alpha, const double *x, double *y, const ApplyRange &rg, cudaStream_t s);
+int launch_nd_hex_apply(b2p_op *op, const int32_t *lidx, double alpha, const double *x, double *y, const ApplyRange &rg, cudaStream_t s,
+                        bool transpose = false);
 int launch_nd_hex_apply4(b2p_op *op, const int32_t *lidx, double alpha, const double *x, double *y, const ApplyRange &rg, cudaStream_t s);
 int launch_nd_hex_apply5(b2p_op *op, const int32_t *lidx, double alpha, const double *x, double *y, const ApplyRange &rg, cudaStream_t s);
 bool nd_hex_apply5_eligible(b2p_op *op);
-int launch_nd_hex_apply6(b2p_op *op, const int32_t *lidx, double alpha, const double *x, double *y, const ApplyRange &rg, cudaStream_t s);
+int launch_nd_hex_apply6(b2p_op *op, const int32_t *lidx, double alpha, const double *x, double *y, const ApplyRange &rg, cudaStream_t s,
+                         bool transpose = false);
 bool nd_hex_apply6_eligible(b2p_op *op);
 bool nd_tables_symmetric(const double *tab, int p, int q, double rel_tol);
-int launch_nd_hex_apply7(b2p_op *op, const int32_t *lidx, double alpha, const double *x, double *y, const ApplyRange &rg, cudaStream_t s);
+int launch_nd_hex_apply7(b2p_op *op, const int32_t *lidx, double alpha, const double *x, double *y, const ApplyRange &rg, cudaStream_t s,
+                         bool transpose = false);
 bool nd_hex_apply7_eligible(b2p_op *op);
 // fused complex apply (b2p_hex_nd4.cu): both parts of a split complex vector in one pass over the geometry
 bool nd_hex_apply4z_eligible(const b2p_op *op);

@@ -147,7 +147,7 @@ public:
   {
     if (!halo) return true;
     for (auto &t : terms)
-      if (t.op->kind == B2P_ND_WEAKCURL || t.op->kind == B2P_ND_MIXEDCURL) return false;
+      if (op_nonsymmetric(t.op)) return false;
     return true;
   }
   void AddMult(const double *x, double *y, double a = 1.0) const override;

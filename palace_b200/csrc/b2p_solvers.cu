@@ -123,8 +123,9 @@ void ParOperator::MultHaloBody(const double *x, double *y, cudaStream_t s) const
   // checks the neighbours' flags just before it reaches the first interface element, so the forward exchange
   // costs nothing on the critical path. (H1 operators use the separate wait kernel.)
   bool in_kernel = h->p2p && ne_interior > 0;
-  // only the sum-factorised ND kernel polls the flags itself; H1 and dense-basis (tet) operators need the separate wait kernel
-  for (auto &t : terms) in_kernel = in_kernel && t.op->kind != B2P_H1_DIFFUSION && !t.op->dense;
+  // only the sum-factorised ND kernel polls the flags itself; H1, dense-basis (tet) and block (mixed curl) operators need the
+  // separate wait kernel
+  for (auto &t : terms) in_kernel = in_kernel && t.op->kind != B2P_H1_DIFFUSION && !t.op->dense && !t.op->bcoef;
   if (fused)
     halo_pre_p2p(h, x, y, height, in_kernel, s);  // forward exchange and both zero-fills: one launch
   else if (h->p2p)
@@ -283,7 +284,7 @@ void ParOperator::Mult(const double *x, double *y) const
 void ParOperator::MultTranspose(const double *x, double *y) const
 {
   bool nonsym = false;
-  for (auto &t : terms) nonsym = nonsym || t.op->kind == B2P_ND_WEAKCURL || t.op->kind == B2P_ND_MIXEDCURL;
+  for (auto &t : terms) nonsym = nonsym || op_nonsymmetric(t.op);
   if (!nonsym)
   {
     Mult(x, y);

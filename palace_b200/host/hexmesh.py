@@ -48,6 +48,11 @@ class HexMesh:
     elems: np.ndarray  # [NE, 8] int64
     attr: np.ndarray  # [NE] int32, 1-based, contiguous (mesh.cpp:46-83)
     warp: object = None  # optional smooth map R^3 -> R^3 applied to all node coordinates
+    # [NE, 8, 3] physical corner coordinates when they are not verts[elems]: a periodic mesh identifies the vertices of
+    # opposite faces in `elems` (the connectivity the spaces are numbered from), while each element keeps its own corners.
+    # Code that takes element positions from verts[elems] (element centroids for partitioning, for instance) sees the top
+    # layer of a periodic mesh folded onto the bottom face: read the corners through node_coords / `corners` instead.
+    corners: np.ndarray = None
 
     @property
     def ne(self):
@@ -69,21 +74,29 @@ class HexMesh:
                     w[a + 2 * b + 4 * c] = (
                         (xi[0] if a else 1 - xi[0]) * (xi[1] if b else 1 - xi[1]) * (xi[2] if c else 1 - xi[2])
                     )
-        vc = self.verts[self.elems]  # [NE, 8, 3]
+        vc = self.verts[self.elems] if self.corners is None else self.corners  # [NE, 8, 3]
         xe = np.einsum("evc,vn->ecn", vc, w)
         if self.warp is not None:
             xe = self.warp(xe)
         return np.ascontiguousarray(xe)
 
 
-def box_mesh(n, size=(1.0, 1.0, 1.0), *, warp_amp=0.0, scramble_seed=None, n_attr=1, origin=(0.0, 0.0, 0.0)) -> HexMesh:
+def box_mesh(n, size=(1.0, 1.0, 1.0), *, warp_amp=0.0, scramble_seed=None, n_attr=1, origin=(0.0, 0.0, 0.0),
+             periodic_z=False) -> HexMesh:
     """Uniform nx*ny*nz box. ``warp_amp`` > 0 applies a smooth non-affine warp to every node
     (SURVEY §8d.2 'smoothly warped variant'); ``scramble_seed`` rotates each element's local frame
     by a random cube symmetry so that edge/face orientation handling is exercised; attributes are
-    striped ``1 + e % n_attr`` (test/unit/test-libceed.cpp:54-64)."""
+    striped ``1 + e % n_attr`` (test/unit/test-libceed.cpp:54-64).
+
+    ``periodic_z``: the unit cell of a structure periodic along z (Floquet-periodic models). The vertices of the top face are
+    the bottom face's in the connectivity, so the two z faces are interior and the spaces are continuous across them; the
+    elements keep their physical corners (``HexMesh.corners``). The warp vanishes on both z faces, so it keeps them matching.
+    Needs nz >= 3: with two layers the vertical edges of both layers would join the same two vertices."""
     if np.isscalar(n):
         n = (int(n),) * 3
     nx, ny, nz = n
+    if periodic_z and nz < 3:
+        raise ValueError(f"periodic_z needs at least 3 element layers along z, got nz = {nz}")
     xs = origin[0] + np.linspace(0, size[0], nx + 1)
     ys = origin[1] + np.linspace(0, size[1], ny + 1)
     zs = origin[2] + np.linspace(0, size[2], nz + 1)
@@ -114,6 +127,11 @@ def box_mesh(n, size=(1.0, 1.0, 1.0), *, warp_amp=0.0, scramble_seed=None, n_att
                             old[perm[d]] = 1 - newc[d] if flips[d] else newc[d]
                         new[sel, a + 2 * b + 4 * c] = elems[sel, old[0] + 2 * old[1] + 4 * old[2]]
         elems = new
+    corners = None
+    if periodic_z:
+        corners = verts[elems]
+        layer = (nx + 1) * (ny + 1)
+        elems = np.where(elems >= nz * layer, elems - nz * layer, elems)  # top vertex layer -> bottom vertex layer
     attr = (1 + (np.arange(elems.shape[0]) % n_attr)).astype(np.int32)
     warp = None
     if warp_amp:
@@ -131,7 +149,7 @@ def box_mesh(n, size=(1.0, 1.0, 1.0), *, warp_amp=0.0, scramble_seed=None, n_att
             out[:, 2] += amp * L[2] * bump * np.cos(1.3 * sx - 0.2)
             return out
 
-    return HexMesh(verts=verts, elems=elems, attr=attr, warp=warp)
+    return HexMesh(verts=verts, elems=elems, attr=attr, warp=warp, corners=corners)
 
 
 def partition_box(n, parts):
