@@ -158,9 +158,10 @@ int b2p_op_apply_add(b2p_op *op, const double *x, double *y, b2p_stream s);
  *   B2P_APPLY_HALFWARP_KERNEL  run the one-element-per-warp ND kernel where it applies (p = 3, q1d = 4,
  *                            mirror-symmetric 1-D tables; ignored otherwise)
  *   B2P_APPLY_ROUND1_KERNEL  run nd_hex_apply4_kernel (the round-1 production kernel) where the default is
- *                            nd_hex_apply6_kernel (p = 2, 3 at q1d = p + 1); same as B2P_ND_KERNEL=4 for one call
+ *                            nd_hex_apply6_kernel (p = 3) or nd_hex_apply7_kernel (p = 2, 4, 5, 6), at q1d = p + 1;
+ *                            same as B2P_ND_KERNEL=4 for one call
  *   B2P_APPLY_CTA_KERNEL     run nd_hex_apply7_kernel (one CTA per element batch, one 1-D line per thread) where it
- *                            applies (p = 4, 5, 6 at q1d = p + 1, mirror-symmetric tables; ignored otherwise); same as
+ *                            applies (p = 2 ... 6 at q1d = p + 1, mirror-symmetric tables; ignored otherwise); same as
  *                            B2P_ND_KERNEL=7 for one call */
 enum
 {

@@ -102,6 +102,7 @@ int apply_range(b2p_op *op, const int32_t *lidx, double alpha, const double *x, 
   // Block operators (mixed curl kinds on hexes and sums containing one): nd_hex_apply6_kernel (p = 2, 3) or
   // nd_hex_apply7_kernel (p = 4, 5, 6) at q1d = p + 1 with mirror-symmetric tables, the cross-check kernel for everything else
   // and whenever an apply flag asks for another kernel (there is no block form in nd_hex_apply4/5_kernel).
+  // B2P_APPLY_CTA_KERNEL / B2P_ND_KERNEL=7 select nd_hex_apply7_kernel at p = 2, 3 too (slower there: DESIGN.md 4.1).
   if (op->bcoef)
   {
     const bool tr = (flags & B2P_APPLY_TRANSPOSE) != 0;
@@ -111,7 +112,8 @@ int apply_range(b2p_op *op, const int32_t *lidx, double alpha, const double *x, 
       return e ? std::atoi(e) : 0;
     }();
     const bool other = (flags & (B2P_APPLY_SIMPLE_KERNEL | B2P_APPLY_ROUND1_KERNEL | B2P_APPLY_HALFWARP_KERNEL)) || forced == 4 || forced == 5;
-    if (!other && nd_hex_apply6_eligible(op)) return launch_nd_hex_apply6(op, lidx, alpha, x, y, rg, s, tr);
+    const bool cta = (flags & B2P_APPLY_CTA_KERNEL) || forced == 7;
+    if (!other && !cta && nd_hex_apply6_eligible(op)) return launch_nd_hex_apply6(op, lidx, alpha, x, y, rg, s, tr);
     if (!other && nd_hex_apply7_eligible(op)) return launch_nd_hex_apply7(op, lidx, alpha, x, y, rg, s, tr);
     return launch_nd_hex_apply(op, lidx, alpha, x, y, rg, s, tr);
   }
@@ -121,8 +123,8 @@ int apply_range(b2p_op *op, const int32_t *lidx, double alpha, const double *x, 
   // One-element-per-warp variant (p = 3, q1d = 4, mirror-symmetric tables): opt-in through the apply flag or
   // B2P_ND_KERNEL=5; slower than nd_hex_apply4_kernel (DESIGN.md 4.1), kept for the analysis.
   // B2P_ND_KERNEL = 4 | 5 | 6 | 7 forces one of the sum-factorised ND kernels; default: the register-gather pipeline
-  // nd_hex_apply6_kernel where it is the faster one (p = 2, 3 at q1d = p + 1; bench.py's round1_kernel_nd_hex_apply4 experiment
-  // times the alternative), nd_hex_apply4_kernel everywhere else.
+  // nd_hex_apply6_kernel at p = 3 (q1d = 4), nd_hex_apply7_kernel at p = 2, 4, 5, 6 (q1d = p + 1), each where it measured
+  // faster (DESIGN.md 4.1, tools/nd7_ab.py), nd_hex_apply4_kernel everywhere else.
   static const int nd_kernel = []
   {
     const char *e = std::getenv("B2P_ND_KERNEL");
@@ -130,15 +132,16 @@ int apply_range(b2p_op *op, const int32_t *lidx, double alpha, const double *x, 
   }();
   if (((flags & B2P_APPLY_HALFWARP_KERNEL) || nd_kernel == 5) && nd_hex_apply5_eligible(op))
     return launch_nd_hex_apply5(op, lidx, alpha, x, y, rg, s);
-  if ((nd_kernel == 6 || nd_kernel == 0) && !(flags & B2P_APPLY_ROUND1_KERNEL) && nd_hex_apply6_eligible(op))
+  if ((nd_kernel == 6 || (nd_kernel == 0 && op->p == 3)) && !(flags & (B2P_APPLY_ROUND1_KERNEL | B2P_APPLY_CTA_KERNEL)) &&
+      nd_hex_apply6_eligible(op))
   {
     static const bool trace = std::getenv("B2P_TRACE_KERNEL") != nullptr;
     if (trace) fprintf(stderr, "[b2p] nd_hex_apply6 p=%d q1d=%d kind=%d ne=%d\n", op->p, op->q1d, op->kind, op->ne);
     return launch_nd_hex_apply6(op, lidx, alpha, x, y, rg, s);
   }
-  // p = 4, 5, 6 at q1d = p + 1: nd_hex_apply7_kernel (one CTA per element batch, warps specialised by vector component, one 1-D
-  // line per thread; faster than nd_hex_apply4_kernel at these orders, tools/nd7_ab.py times both). B2P_ND_KERNEL=4 or
-  // B2P_APPLY_ROUND1_KERNEL select the round-1 kernel.
+  // p = 2 ... 6 at q1d = p + 1: nd_hex_apply7_kernel (one CTA per element batch, warps specialised by vector component, one 1-D
+  // line per thread; tools/nd7_ab.py times its shapes against nd_hex_apply4_kernel). B2P_APPLY_CTA_KERNEL / B2P_ND_KERNEL=7 select
+  // it at p = 3 too; B2P_ND_KERNEL=4 or B2P_APPLY_ROUND1_KERNEL select the round-1 kernel.
   if (((flags & B2P_APPLY_CTA_KERNEL) || nd_kernel == 7 || nd_kernel == 0) && !(flags & B2P_APPLY_ROUND1_KERNEL) && nd_hex_apply7_eligible(op))
   {
     static const bool trace = std::getenv("B2P_TRACE_KERNEL") != nullptr;

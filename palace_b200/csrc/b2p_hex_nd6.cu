@@ -212,13 +212,14 @@ __global__ void __launch_bounds__(NW * 32, MINB) nd_hex_apply6_kernel(const __gr
   }
   __syncwarp();
 
+  const uint64_t once = l2_evict_first_policy();  // the bulk copies below stream data read once per launch
   auto issue_ring = [&](int bb, int slot)
   {
     const int e0 = bb * NEW, nel = min(NEW, prm.ne - e0);
     const uint32_t ib = (uint32_t)(nel * PS * sizeof(int32_t)), cb = (uint32_t)(nel * CE * sizeof(double));
     mbar_expect_tx(bar_i + slot, ib + cb);
-    tma_bulk_g2s(sR + slot * L::SLOT, prm.lidx + (size_t)e0 * PS, ib, bar_i + slot);
-    tma_bulk_g2s(sR + slot * L::SLOT + L::SLOT_I, prm.ecoef + (size_t)e0 * CE, cb, bar_i + slot);
+    tma_bulk_g2s_hint(sR + slot * L::SLOT, prm.lidx + (size_t)e0 * PS, ib, bar_i + slot, once);
+    tma_bulk_g2s_hint(sR + slot * L::SLOT + L::SLOT_I, prm.ecoef + (size_t)e0 * CE, cb, bar_i + slot, once);
   };
   auto prefetch_geom = [&](int bb)
   {
@@ -238,7 +239,7 @@ __global__ void __launch_bounds__(NW * 32, MINB) nd_hex_apply6_kernel(const __gr
     const int e0 = bb * NEW, nel = min(NEW, prm.ne - e0);
     const uint32_t bytes = (uint32_t)(nel * GE * sizeof(double));
     mbar_expect_tx(bar_g, bytes);
-    tma_bulk_g2s(sG, prm.qd + (size_t)e0 * GE, bytes, bar_g);
+    tma_bulk_g2s_hint(sG, prm.qd + (size_t)e0 * GE, bytes, bar_g, once);
   };
 
   // x values of the batch whose Z phase comes next, in the registers of the lane that contracts them; `xsign` holds the

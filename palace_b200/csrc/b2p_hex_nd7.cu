@@ -1,10 +1,11 @@
 // High-order Nedelec hexahedron apply kernel: one CTA per element batch, one 1-D line per thread.
 //
-//   y_L += alpha * sum_e E_e^T  B^T  D  B  E_e x_L          (curl-curl, mass, curl-curl + mass),   p = 4, 5, 6 at q1d = p + 1
+//   y_L += alpha * sum_e E_e^T  B^T  D  B  E_e x_L          (curl-curl, mass, curl-curl + mass),   p = 2 ... 6 at q1d = p + 1
 //
-// Same operator as nd_hex_apply4_kernel / nd_hex_apply6_kernel. Those give every WARP whole elements and keep a
-// (qy,qz) line of u, curl u in registers through the pointwise D; at p >= 5 a lane then owns several lines
-// (q1d^2 = 36, 49 > 32), the kernels spill and 3-5 warps fit an SM (0.19 / 0.12 of the HBM roofline at p = 5 / 6).
+// Same operator as nd_hex_apply4_kernel. That kernel gives every WARP whole elements and keeps a (qy,qz) line of u, curl u
+// in registers through the pointwise D; at p >= 5 a lane then owns several lines (q1d^2 = 36, 49 > 32), the kernel spills
+// and 3-5 warps fit an SM (0.19 / 0.12 of the HBM roofline at p = 5 / 6); at p = 2, 3 its registers and shared memory
+// hold it to 8 warps per SM, too few to hide the latency of its dependent FP64 chains.
 // Here the CTA owns the batch and the warps are specialised by vector COMPONENT (x-, y-, z-directed dofs):
 //   * every phase is a set of independent 1-D contractions ("lines"); a thread owns ONE line of its component, so
 //     its live state is one input line, one or two output lines and the table entries in flight (<= 85 registers,
@@ -219,10 +220,11 @@ __global__ void __launch_bounds__(3 * WPC * 32, MINB) nd_hex_apply7_kernel(const
 
   auto issue_geom = [&](int bb)  // (one thread)
   {
+    const uint64_t once = l2_evict_first_policy();  // q-data and coefficient blocks are read once per launch
     const int e0 = bb * NE, nel = min(NE, prm.ne - e0);
     mbar_expect_tx(bar_g, (uint32_t)(nel * (L::GE + L::CE) * sizeof(double)));
-    tma_bulk_g2s(sG, prm.qd + (size_t)e0 * L::GE, (uint32_t)(nel * L::GE * sizeof(double)), bar_g);
-    tma_bulk_g2s(sC, prm.ecoef + (size_t)e0 * L::CE, (uint32_t)(nel * L::CE * sizeof(double)), bar_g);
+    tma_bulk_g2s_hint(sG, prm.qd + (size_t)e0 * L::GE, (uint32_t)(nel * L::GE * sizeof(double)), bar_g, once);
+    tma_bulk_g2s_hint(sC, prm.ecoef + (size_t)e0 * L::CE, (uint32_t)(nel * L::CE * sizeof(double)), bar_g, once);
   };
   uint32_t par_g = 0;
   if (GSM)
@@ -755,25 +757,39 @@ __global__ void __launch_bounds__(3 * WPC * 32, MINB) nd_hex_apply7_kernel(const
 }
 
 // Launch shape per order: elements per batch, warps per component, CTAs per SM (register cap 65536 / threads per SM), q-data
-// staged by TMA, component-wide barriers; chosen by A/B timing of the shapes (tools/nd7_ab.py, B2P_ND7_CFG).
+// staged by TMA, component-wide barriers; chosen by A/B timing of the shapes (tools/nd7_ab.py, B2P_ND7_CFG). MINB_BLOCK is the
+// CTAs per SM of the B2P_ND_BLOCK instantiation, whose four-tensor D phase needs more registers than the cap of MINB allows at
+// p = 2, 3.
 template <int P_>
 struct ND7Shape;
 template <>
+struct ND7Shape<2>
+{
+  static constexpr int NE = 3, WPC = 1, MINB = 8, MINB_BLOCK = 4;  // 27 of 32 lanes, 96 threads
+  static constexpr bool GSM = true, CBAR = true;
+};
+template <>
+struct ND7Shape<3>
+{
+  static constexpr int NE = 2, WPC = 1, MINB = 8, MINB_BLOCK = 5;  // 32 of 32 lanes, 96 threads
+  static constexpr bool GSM = true, CBAR = true;
+};
+template <>
 struct ND7Shape<4>
 {
-  static constexpr int NE = 1, WPC = 1, MINB = 8;  // 25 of 32 lanes, 96 threads
+  static constexpr int NE = 1, WPC = 1, MINB = 8, MINB_BLOCK = MINB;  // 25 of 32 lanes, 96 threads
   static constexpr bool GSM = true, CBAR = true;
 };
 template <>
 struct ND7Shape<5>
 {
-  static constexpr int NE = 2, WPC = 3, MINB = 2;  // 72 of 96 lanes, 288 threads
+  static constexpr int NE = 2, WPC = 3, MINB = 2, MINB_BLOCK = MINB;  // 72 of 96 lanes, 288 threads
   static constexpr bool GSM = true, CBAR = true;
 };
 template <>
 struct ND7Shape<6>
 {
-  static constexpr int NE = 1, WPC = 2, MINB = 3;  // 49 of 64 lanes, 192 threads
+  static constexpr int NE = 1, WPC = 2, MINB = 3, MINB_BLOCK = MINB;  // 49 of 64 lanes, 192 threads
   static constexpr bool GSM = true, CBAR = true;
 };
 
@@ -854,6 +870,14 @@ int launch7(b2p_op *op, const int32_t *lidx, double alpha, const double *x, doub
     return (code % 10) == 2   ? launch7_cfg<P_, KIND, NEV, (P_ == PP ? WPCV : S::WPC), MB, true, true>(op, lidx, alpha, x, y, rg, s)   \
            : (code % 10) == 1 ? launch7_cfg<P_, KIND, NEV, (P_ == PP ? WPCV : S::WPC), MB, true, false>(op, lidx, alpha, x, y, rg, s)  \
                               : launch7_cfg<P_, KIND, NEV, (P_ == PP ? WPCV : S::WPC), MB, false, false>(op, lidx, alpha, x, y, rg, s);
+    if constexpr (P_ == 2)
+    {
+      B2P_CFG(2, 3, 1, 7) B2P_CFG(2, 3, 1, 8) B2P_CFG(2, 3, 1, 9) B2P_CFG(2, 7, 2, 4)
+    }
+    if constexpr (P_ == 3)
+    {
+      B2P_CFG(3, 2, 1, 7) B2P_CFG(3, 2, 1, 8) B2P_CFG(3, 2, 1, 9) B2P_CFG(3, 3, 2, 4) B2P_CFG(3, 4, 2, 4)
+    }
     if constexpr (P_ == 4)
     {
       B2P_CFG(4, 1, 1, 6) B2P_CFG(4, 1, 1, 8) B2P_CFG(4, 2, 2, 4) B2P_CFG(4, 5, 4, 2)
@@ -868,7 +892,8 @@ int launch7(b2p_op *op, const int32_t *lidx, double alpha, const double *x, doub
     }
 #undef B2P_CFG
   }
-  return launch7_cfg<P_, KIND, S::NE, S::WPC, S::MINB, S::GSM, S::CBAR>(op, lidx, alpha, x, y, rg, s, transpose);
+  constexpr int MINB = KIND == B2P_ND_BLOCK ? S::MINB_BLOCK : S::MINB;
+  return launch7_cfg<P_, KIND, S::NE, S::WPC, MINB, S::GSM, S::CBAR>(op, lidx, alpha, x, y, rg, s, transpose);
 }
 
 }  // namespace
@@ -876,7 +901,7 @@ int launch7(b2p_op *op, const int32_t *lidx, double alpha, const double *x, doub
 bool nd_hex_apply7_eligible(b2p_op *op)
 {
   if (!op || op->dense || op->assembled || op->kind == B2P_H1_DIFFUSION || !(op->ecoef || op->bcoef)) return false;
-  if (!(op->q1d == op->p + 1 && op->p >= 4 && op->p <= 6)) return false;
+  if (!(op->q1d == op->p + 1 && op->p >= 2 && op->p <= 6)) return false;
   // The kernel reads mirrored table entries through one stored value. Tables evaluated in floating point (MFEM's, or
   // tests/hexspace.py) mirror to a few ulp of the LARGEST entry (measured 6e-16 ... 9e-16 at p = 4, 5): the substitution
   // changes the operator by less than the tables' own rounding.
@@ -898,6 +923,8 @@ int launch_nd_hex_apply7(b2p_op *op, const int32_t *lidx, double alpha, const do
       case B2P_CURLCURL_MASS: return launch7<PP, B2P_CURLCURL_MASS>(op, lidx, alpha, x, y, rg, s);                    \
     }                                                                                                                 \
   }
+  B2P_CASE(2)
+  B2P_CASE(3)
   B2P_CASE(4)
   B2P_CASE(5)
   B2P_CASE(6)

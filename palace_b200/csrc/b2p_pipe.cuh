@@ -11,6 +11,11 @@ namespace b2p
 inline void mbar_init(uint64_t *bar, int count) { ::cuda_emu::mbar_init(bar, count); }
 inline void mbar_expect_tx(uint64_t *bar, uint32_t bytes) { ::cuda_emu::mbar_expect_tx(bar, bytes); }
 inline void tma_bulk_g2s(void *dst, const void *src, uint32_t bytes, uint64_t *bar) { ::cuda_emu::tma_bulk_g2s(dst, src, bytes, bar); }
+inline uint64_t l2_evict_first_policy() { return 0; }
+inline void tma_bulk_g2s_hint(void *dst, const void *src, uint32_t bytes, uint64_t *bar, uint64_t)
+{
+  ::cuda_emu::tma_bulk_g2s(dst, src, bytes, bar);
+}
 inline void mbar_wait(uint64_t *bar, uint32_t parity) { ::cuda_emu::mbar_wait(bar, parity); }
 inline void cp_async8(void *dst, const void *src) { ::cuda_emu::cp_async(dst, src, 8); }
 inline void cp_async_commit() { ::cuda_emu::cp_async_commit(); }
@@ -53,6 +58,22 @@ __device__ __forceinline__ void tma_bulk_g2s(void *dst, const void *src, uint32_
 {
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(smem_u32(dst)),
                "l"(src), "r"(bytes), "r"(smem_u32(bar))
+               : "memory");
+}
+// L2 policy for data an element kernel reads exactly once per launch (q-data, restriction indices, coefficient blocks):
+// their lines are evicted first, so the stream does not push out the lines that are used again -- x and y, which every
+// element around a dof gathers and scatter-adds, and whatever the caller keeps in L2 between launches.
+__device__ __forceinline__ uint64_t l2_evict_first_policy()
+{
+  uint64_t pol;
+  asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));
+  return pol;
+}
+__device__ __forceinline__ void tma_bulk_g2s_hint(void *dst, const void *src, uint32_t bytes, uint64_t *bar, uint64_t policy)
+{
+  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;" ::"r"(
+                   smem_u32(dst)),
+               "l"(src), "r"(bytes), "r"(smem_u32(bar)), "l"(policy)
                : "memory");
 }
 __device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity)

@@ -35,7 +35,7 @@ from palace_b200.host import coeff as cf  # noqa: E402
 from palace_b200.host import hexmesh as hm  # noqa: E402
 from tests import common  # noqa: E402
 
-BOX = {3: 29, 6: 15}  # elements per side of the z-periodic box: 2.01M ND dofs at p = 3, 2.22M at p = 6
+BOX = {2: 43, 3: 29, 6: 15}  # elements per side of the z-periodic box: 1.94M ND dofs at p = 2, 2.01M at p = 3, 2.22M at p = 6
 
 
 def terms(kz, sigma):

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""A/B of the high-order hexahedron kernels on one GPU: nd_hex_apply4_kernel (warp per element) against
+"""A/B of the sum-factorised ND hexahedron kernels on one GPU: nd_hex_apply4_kernel (warp per element) against
 nd_hex_apply7_kernel (CTA per element batch) in its launch shapes (B2P_ND7_CFG), curl-curl + mass, isotropic
 coefficient, L2 flushed between launches. One JSON line per (order, variant): kernel time, GDoF/s, fraction of the
 measured HBM peak on bench.py's byte model, and the largest relative difference to nd_hex_apply4_kernel's result."""
@@ -19,9 +19,11 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--orders", default="4,5,6")
     ap.add_argument("--reps", type=int, default=30)
-    ap.add_argument("--configs", default="4:118g,118c,542c;5:232g,232c,341c;6:123g,123c,122c",
+    ap.add_argument("--configs", default="2:317c,318g,318c,319c,724c;3:217c,218g,218c,219c,324c,424c;4:118g,118c,542c;5:232g,232c,341c;6:123g,123c,122c",
                     help="B2P_ND7_CFG values per order: <elements per batch><warps per component><CTAs per SM><d|g|c>")
     ap.add_argument("--skip-round1", action="store_true")
+    ap.add_argument("--default-arm", action="store_true",
+                    help="also time the call without kernel flags (the kernel B2P_ND_KERNEL selects, or the default)")
     ap.add_argument("--warp", type=float, default=0.0)
     ap.add_argument("--coefficient", default="iso")
     args = ap.parse_args()
@@ -74,6 +76,8 @@ def main():
 
         if not args.skip_round1:
             run("nd_hex_apply4_kernel", round1_kernel=True)
+        if args.default_arm:
+            run("default B2P_ND_KERNEL=" + os.environ.get("B2P_ND_KERNEL", "0"))
         cfgs = dict(part.split(":") for part in args.configs.split(";"))
         for cfg in cfgs.get(str(p), "").split(","):
             if not cfg:
