@@ -268,7 +268,9 @@ void b2p_halo_destroy(b2p_halo *h);
  *   CeedOperatorLinearAssembleSymbolic + COO->CSR sort). Any operator on the same space can be assembled into it.
  * b2p_csr_assemble: numeric phase on the device, values = sum_t coefs[t] * A_t (the reference's "set" = false
  *   accumulation). The element matrices come from the operator kernels themselves (applied to local unit vectors
- *   through an identity restriction), so hex / tet / assembled-D operators are all covered; no host work, no sort.
+ *   through an identity restriction), so hex / tet / assembled-D operators are all covered; no host work, no sort. Column j
+ *   of every element matrix is the apply to e_j, so the non-symmetric hex kinds (B2P_ND_WEAKCURL / B2P_ND_MIXEDCURL) and
+ *   block sums that contain them are assembled as A, not A^T.
  * b2p_csr_device_arrays: rowptr[n+1] / col[nnz] (int32, sorted columns) / val[nnz] device pointers, owned by the handle
  *   (wrap them in a hypre_CSRMatrix). b2p_csr_eliminate: essential rows/columns as HypreParMatrix::EliminateBC with
  *   the ParOperator diagonal policy (1 = DIAG_ONE, 0 = DIAG_ZERO), for callers that skip the P^T A P step.
@@ -458,6 +460,27 @@ void b2p_coperator_destroy(b2p_coperator *A);
 /* A real preconditioner (any b2p_solver, e.g. the multigrid) applied to the real and imaginary parts: the
  * "PCMatReal" configuration (models/spaceoperator.cpp:1098-1105, utils/configfile.hpp:1051). */
 int b2p_csolver_real_pc(b2p_ctx *ctx, b2p_solver *real_pc, b2p_csolver **out);
+/* MfemWrapperSolver<ComplexOperator> (linalg/solver.cpp:33-177; single partition): a complex solver that runs a REAL solver on
+ * the device-assembled matrix of the complex operator given to b2p_csolver_set_operator -- the coarse solver of the complex
+ * multigrid (b2p_csolver_gmg hands it A[0]). The operator must be a b2p_coperator_par, or a b2p_coperator_wrap whose parts are
+ * single-partition b2p_operator_par on one space; anything else fails at set_operator with b2p_last_error set. Both parts are
+ * assembled on one CSR pattern (Ar eliminated with the operator's diagonal policy, Ai with DIAG_ZERO), then
+ *   complex_matrix == 0: the inner solver gets Ar + Ai, and mult applies it to the real and the imaginary part separately;
+ *   complex_matrix != 0: the inner solver gets the 2n block [[Ar, Ai], [Ai, -Ar]] (applied from the two value arrays, not
+ *                        formed) and mult solves it once for [xr; -xi] with the right-hand side [br; bi].
+ * With only one part present (no imaginary or no real coefficient, a NULL part) that part alone is the matrix. Takes over
+ * `inner` (Krylov or smoother) and, optionally, its preconditioner `inner_pc`, which also gets the matrix; both handles then
+ * only need b2p_solver_destroy. mult honours b2p_csolver_set_initial_guess. After b2p_coperator_set_coefficients the next
+ * set_operator with the same operator re-assembles the values only (no new symbolic phase).
+ * b2p_csolver_assembled_nnz: entries of the real matrix the inner solver sees (4 x the pattern for the block form); s is the
+ * solver, or the complex multigrid that took it over; -1 before set_operator.
+ * b2p_csolver_assembled_device_arrays: rows, entries and device rowptr[rows+1] / col[nnz] (int32, sorted columns) / val[nnz] of
+ * that matrix, owned by the solver and valid until its next set_operator: the input of a sparse direct solver. The explicit
+ * block matrix is built on the first request (pattern on the host once, values by a kernel). */
+int b2p_csolver_assembled(b2p_ctx *ctx, b2p_solver *inner, b2p_solver *inner_pc, int complex_matrix, b2p_csolver **out);
+int64_t b2p_csolver_assembled_nnz(b2p_csolver *s);
+int b2p_csolver_assembled_device_arrays(b2p_csolver *s, int64_t *rows, int64_t *nnz, const int32_t **rowptr, const int32_t **col,
+                                        const double **val);
 /* CgSolver / GmresSolver / FgmresSolver<ComplexOperator> (linalg/iterative.cpp:361-871; type 0/1/2) */
 /* JacobiSmoother<ComplexOperator> (linalg/jacobi.cpp:75-105): y = omega D^-1 x with the complex diagonal of the operator given to
  * b2p_csolver_set_operator; omega != 0. The preconditioner of the complex-valued (PCMatReal = false) path. */

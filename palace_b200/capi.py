@@ -444,6 +444,22 @@ class Csr:
             self.h = None
 
 
+def _device_view(ptr, n, ctype):
+    """1-D tensor viewing n elements of library-owned device memory (no copy)."""
+    import torch
+
+    dtype = np.dtype(ctype)
+    if torch.cuda.device_count() > 0:
+        class _Cai:  # __cuda_array_interface__ lets torch wrap a raw device pointer
+            pass
+
+        o = _Cai()
+        o.__cuda_array_interface__ = {"shape": (int(n),), "typestr": dtype.str, "data": (int(ptr or 0), False), "version": 2}
+        return torch.as_tensor(o, device="cuda")
+    # no CUDA device: the library is the host-thread emulation build, whose device memory is host memory
+    return torch.from_numpy(np.ctypeslib.as_array(C.cast(ptr, C.POINTER(ctype)), shape=(int(n),)))
+
+
 def set_stream(ctx, stream=None):
     _chk(lib().b2p_ctx_set_stream(ctx.h, _stream(stream)), ctx.h)
 
@@ -780,6 +796,34 @@ class ComplexSolver:
         s = cls(ctx, h)
         s._keep.append(real_solver)
         return s
+
+    @classmethod
+    def assembled(cls, ctx, inner: Solver, inner_pc: Solver = None, complex_matrix=False):
+        """Coarse solver on the device-assembled matrix of the complex operator given to set_operator
+        (MfemWrapperSolver<ComplexOperator>): the real solver ``inner`` (taken over, with its preconditioner ``inner_pc``) runs
+        on Ar + Ai for each part, or with ``complex_matrix`` once on the real 2n block [[Ar, Ai], [Ai, -Ar]]."""
+        h = C.c_void_p()
+        _chk(lib().b2p_csolver_assembled(ctx.h, inner.h, inner_pc.h if inner_pc is not None else None, int(bool(complex_matrix)),
+                                         C.byref(h)), ctx.h)
+        s = cls(ctx, h)
+        s._keep += [inner, inner_pc]
+        return s
+
+    def assembled_nnz(self):
+        """Entries of the real matrix the inner solver sees (this solver or the multigrid that took it over); -1 before set_operator."""
+        f = lib().b2p_csolver_assembled_nnz
+        f.restype = C.c_int64
+        return int(f(self.h))
+
+    def assembled_device_arrays(self):
+        """(rowptr, col, val) of the real matrix the inner solver sees, as tensors viewing the solver's device memory (valid until
+        its next set_operator): int32 rowptr[rows + 1], int32 col[nnz], float64 val[nnz]."""
+        rows, nnz = C.c_int64(), C.c_int64()
+        rp, cl, vl = C.c_void_p(), C.c_void_p(), C.c_void_p()
+        _chk(lib().b2p_csolver_assembled_device_arrays(self.h, C.byref(rows), C.byref(nnz), C.byref(rp), C.byref(cl), C.byref(vl)),
+             self.ctx.h)
+        return (_device_view(rp.value, rows.value + 1, C.c_int32), _device_view(cl.value, nnz.value, C.c_int32),
+                _device_view(vl.value, nnz.value, C.c_double))
 
     @classmethod
     def gmg(cls, ctx, coarse, P, G=None, cycle_it=1, smooth_it=1, cheby_order=4, sf_max=1.0):

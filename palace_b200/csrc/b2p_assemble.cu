@@ -74,6 +74,68 @@ __global__ void csr_diag_kernel(int64_t n, const int32_t *__restrict__ rowptr, c
     if (col[k] == r) s = val[k];
   d[r] = s;
 }
+// The real 2n x 2n form [[Ar, Ai], [Ai, -Ar]] of a complex matrix whose parts share one pattern, applied without forming it:
+// x = [u; w] -> y = [Ar u + Ai w; Ai u - Ar w]. One pass over rowptr / col serves both halves (4 + 8 + 8 bytes per nonzero
+// pair, against 2 x (4 + 8) x 2 for the explicit block matrix); lanes as in csr_mult_kernel.
+__global__ void csr_block2_mult_kernel(int64_t n, const int32_t *__restrict__ rowptr, const int32_t *__restrict__ col,
+                                       const double *__restrict__ vr, const double *__restrict__ vi, const double *__restrict__ x,
+                                       double *__restrict__ y)
+{
+  const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const int64_t r = t / CSR_LANES;
+  const int sub = (int)(t % CSR_LANES);
+  double top = 0.0, bot = 0.0;
+  if (r < n)
+    for (int32_t k = rowptr[r] + sub; k < rowptr[r + 1]; k += CSR_LANES)
+    {
+      const int32_t c = col[k];
+      const double ar = vr[k], ai = vi[k], u = x[c], w = x[n + c];
+      top += ar * u + ai * w;
+      bot += ai * u - ar * w;
+    }
+#pragma unroll
+  for (int o = CSR_LANES / 2; o > 0; o >>= 1)
+  {
+    top += __shfl_xor_sync(0xffffffffu, top, o);
+    bot += __shfl_xor_sync(0xffffffffu, bot, o);
+  }
+  if (r < n && sub == 0)
+  {
+    y[r] = top;
+    y[n + r] = bot;
+  }
+}
+// d = [diag Ar; -diag Ar]
+__global__ void csr_block2_diag_kernel(int64_t n, const int32_t *__restrict__ rowptr, const int32_t *__restrict__ col,
+                                       const double *__restrict__ vr, double *__restrict__ d)
+{
+  const int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= n) return;
+  double s = 0.0;
+  for (int32_t k = rowptr[r]; k < rowptr[r + 1]; k++)
+    if (col[k] == r) s = vr[k];
+  d[r] = s;
+  d[n + r] = -s;
+}
+// Values of the explicit block matrix on the pattern of csr_block2_pattern: top row r holds Ar(r, :) then Ai(r, :) (columns
+// c, then n + c), bottom row n + r holds Ai(r, :) then -Ar(r, :).
+__global__ void csr_block2_fill_kernel(int64_t n, int64_t nnz, const int32_t *__restrict__ rowptr, const double *__restrict__ vr,
+                                       const double *__restrict__ vi, double *__restrict__ v2)
+{
+  const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const int64_t r = t / CSR_LANES;
+  const int sub = (int)(t % CSR_LANES);
+  if (r >= n) return;
+  const int32_t b = rowptr[r], e = rowptr[r + 1];
+  for (int32_t k = b + sub; k < e; k += CSR_LANES)
+  {
+    const double ar = vr[k], ai = vi[k];
+    v2[(int64_t)b + k] = ar;
+    v2[(int64_t)e + k] = ai;
+    v2[2 * nnz + b + k] = ai;
+    v2[2 * nnz + e + k] = -ar;
+  }
+}
 // mfem::HypreParMatrix::EliminateBC semantics on the local matrix: essential rows and columns zeroed, diagonal set to
 // one (DIAG_ONE) or zero (DIAG_ZERO)  (rap.cpp:141-146)
 __global__ void csr_eliminate_kernel(int64_t n, const int32_t *__restrict__ rowptr, const int32_t *__restrict__ col, double *val,
@@ -91,6 +153,133 @@ __global__ void mark_kernel(const int32_t *__restrict__ idx, int64_t n, char *fl
 }
 inline unsigned blocks(int64_t n, int nt) { return (unsigned)((n + nt - 1) / nt); }
 }  // namespace
+
+double *csr_values(b2p_csr *A) { return A->d_val; }
+
+// values = sum_t coefs[t] * A_t  (all terms on the space the pattern was built from)
+int csr_assemble_values(b2p_csr *A, int n_terms, b2p_op *const *ops, const double *coefs, double *val, cudaStream_t s)
+{
+  if (!A || !ops || !coefs || !val || n_terms <= 0) return B2P_ERR_ARG;
+  b2p_ctx *ctx = A->ctx;
+  const int64_t nE = (int64_t)A->ne * A->P;
+  B2P_CUDA(ctx, cudaMemsetAsync(val, 0, sizeof(double) * std::max<int64_t>(A->nnz, 1), s));
+  for (int t = 0; t < n_terms; t++)
+  {
+    b2p_op *op = ops[t];
+    B2P_CHECK(ctx, op && op->ne == A->ne && op->P == A->P && op->PS == A->PS && op->lsize == A->n, B2P_ERR_ARG,
+              "b2p_csr_assemble: term %d lives on another space", t);
+    if (coefs[t] == 0.0) continue;
+    // Column j of every element matrix is A_e e_j; it lands at pos(e, i, j) for every row i, so non-symmetric operators (the
+    // mixed curl kinds, block sums) are assembled as they are applied, not as their transpose.
+    for (int j = 0; j < A->P; j++)
+    {
+      B2P_LAUNCH(set_unit_kernel, blocks(nE, 256), 256, 0, s, A->d_x, nE, A->P, j);
+      B2P_CUDA(ctx, cudaMemsetAsync(A->d_y, 0, sizeof(double) * nE, s));
+      ApplyRange rg;
+      rg.n_owned = nE;  // the whole E-vector is "owned": no ghost segment (nE >= the operator's L-size)
+      int rc = apply_range(op, A->d_eidx, 1.0, A->d_x, A->d_y, rg, 0, s);
+      if (rc) return rc;
+      B2P_LAUNCH(scatter_column_kernel, blocks(nE, 256), 256, 0, s, A->d_y, A->d_pos, A->d_gidx, nE, A->P, A->PS, j, coefs[t], val);
+    }
+  }
+  B2P_CUDA(ctx, cudaGetLastError());
+  return B2P_SUCCESS;
+}
+
+int csr_eliminate_values(b2p_csr *A, const int32_t *ess_dofs, int64_t n_ess, int diag_policy, double *val, cudaStream_t s)
+{
+  if (!A || !val || (n_ess > 0 && !ess_dofs)) return B2P_ERR_ARG;
+  if (n_ess <= 0) return B2P_SUCCESS;
+  b2p_ctx *ctx = A->ctx;
+  for (int64_t i = 0; i < n_ess; i++)
+    B2P_CHECK(ctx, ess_dofs[i] >= 0 && ess_dofs[i] < A->n, B2P_ERR_ARG, "b2p_csr_eliminate: essential dof %d outside the matrix", ess_dofs[i]);
+  int32_t *d_ess = nullptr;
+  char *d_flag = nullptr;
+  int rc = upload(ctx, ess_dofs, (size_t)n_ess, &d_ess);
+  if (rc) return rc;
+  if (cudaMalloc(&d_flag, (size_t)A->n) != cudaSuccess)
+  {
+    cudaFree(d_ess);
+    set_error(ctx, "b2p_csr_eliminate: out of device memory");
+    return B2P_ERR_CUDA;
+  }
+  cudaMemsetAsync(d_flag, 0, (size_t)A->n, s);
+  B2P_LAUNCH(mark_kernel, blocks(n_ess, 256), 256, 0, s, d_ess, n_ess, d_flag);
+  B2P_LAUNCH(csr_eliminate_kernel, blocks(A->n, 256), 256, 0, s, A->n, A->d_rowptr, A->d_col, val, d_flag, diag_policy == 1 ? 1 : 0);
+  cudaStreamSynchronize(s);
+  cudaFree(d_ess);
+  cudaFree(d_flag);
+  B2P_CUDA(ctx, cudaGetLastError());
+  return B2P_SUCCESS;
+}
+
+int csr_mult_values(b2p_csr *A, const double *val, const double *x, double *y, cudaStream_t s)
+{
+  if (!A || !val || !x || !y) return B2P_ERR_ARG;
+  B2P_LAUNCH(csr_mult_kernel, blocks(A->n * CSR_LANES, 256), 256, 0, s, A->n, A->d_rowptr, A->d_col, val, x, y);
+  B2P_CUDA(A->ctx, cudaGetLastError());
+  return B2P_SUCCESS;
+}
+
+int csr_diag_values(b2p_csr *A, const double *val, double *d, cudaStream_t s)
+{
+  if (!A || !val || !d) return B2P_ERR_ARG;
+  B2P_LAUNCH(csr_diag_kernel, blocks(A->n, 256), 256, 0, s, A->n, A->d_rowptr, A->d_col, val, d);
+  B2P_CUDA(A->ctx, cudaGetLastError());
+  return B2P_SUCCESS;
+}
+
+int csr_block2_mult(b2p_csr *A, const double *vr, const double *vi, const double *x, double *y, cudaStream_t s)
+{
+  if (!A || !vr || !vi || !x || !y) return B2P_ERR_ARG;
+  B2P_LAUNCH(csr_block2_mult_kernel, blocks(A->n * CSR_LANES, 256), 256, 0, s, A->n, A->d_rowptr, A->d_col, vr, vi, x, y);
+  B2P_CUDA(A->ctx, cudaGetLastError());
+  return B2P_SUCCESS;
+}
+
+int csr_block2_diag(b2p_csr *A, const double *vr, double *d, cudaStream_t s)
+{
+  if (!A || !vr || !d) return B2P_ERR_ARG;
+  B2P_LAUNCH(csr_block2_diag_kernel, blocks(A->n, 256), 256, 0, s, A->n, A->d_rowptr, A->d_col, vr, d);
+  B2P_CUDA(A->ctx, cudaGetLastError());
+  return B2P_SUCCESS;
+}
+
+int csr_block2_pattern(b2p_csr *A, int32_t **rowptr2, int32_t **col2)
+{
+  if (!A || !rowptr2 || !col2) return B2P_ERR_ARG;
+  b2p_ctx *ctx = A->ctx;
+  const int64_t n = A->n, nnz = A->nnz;
+  B2P_CHECK(ctx, 4 * nnz < 2147483647LL, B2P_ERR_UNSUPPORTED, "csr_block2_pattern: %lld entries need 64-bit row pointers",
+            (long long)(4 * nnz));
+  std::vector<int32_t> rp((size_t)2 * n + 1), cl((size_t)4 * nnz);
+  for (int64_t r = 0; r < n; r++)
+  {
+    const int32_t b = A->h_rowptr[(size_t)r], e = A->h_rowptr[(size_t)r + 1];
+    rp[(size_t)r] = 2 * b;
+    rp[(size_t)(n + r)] = (int32_t)(2 * nnz + 2 * b);
+    for (int32_t k = b; k < e; k++)
+    {
+      const int32_t c = A->h_col[(size_t)k];
+      cl[(size_t)b + k] = c;
+      cl[(size_t)e + k] = (int32_t)(n + c);
+      cl[(size_t)(2 * nnz + b + k)] = c;
+      cl[(size_t)(2 * nnz + e + k)] = (int32_t)(n + c);
+    }
+  }
+  rp[(size_t)2 * n] = (int32_t)(4 * nnz);
+  int rc = upload(ctx, rp.data(), rp.size(), rowptr2);
+  if (!rc) rc = upload(ctx, cl.data(), cl.size(), col2);
+  return rc;
+}
+
+int csr_block2_fill(b2p_csr *A, const double *vr, const double *vi, double *val2, cudaStream_t s)
+{
+  if (!A || !vr || !vi || !val2) return B2P_ERR_ARG;
+  B2P_LAUNCH(csr_block2_fill_kernel, blocks(A->n * CSR_LANES, 256), 256, 0, s, A->n, A->nnz, A->d_rowptr, vr, vi, val2);
+  B2P_CUDA(A->ctx, cudaGetLastError());
+  return B2P_SUCCESS;
+}
 }  // namespace b2p
 
 using namespace b2p;
@@ -196,30 +385,7 @@ int b2p_csr_create(b2p_ctx *ctx, b2p_op *op, b2p_csr **out)
 // values = sum_t coefs[t] * A_t  (all terms on the space the pattern was built from)
 int b2p_csr_assemble(b2p_csr *A, int n_terms, b2p_op *const *ops, const double *coefs, b2p_stream stream)
 {
-  if (!A || !ops || !coefs || n_terms <= 0) return B2P_ERR_ARG;
-  b2p_ctx *ctx = A->ctx;
-  cudaStream_t s = (cudaStream_t)stream;
-  const int64_t nE = (int64_t)A->ne * A->P;
-  B2P_CUDA(ctx, cudaMemsetAsync(A->d_val, 0, sizeof(double) * std::max<int64_t>(A->nnz, 1), s));
-  for (int t = 0; t < n_terms; t++)
-  {
-    b2p_op *op = ops[t];
-    B2P_CHECK(ctx, op && op->ne == A->ne && op->P == A->P && op->PS == A->PS && op->lsize == A->n, B2P_ERR_ARG,
-              "b2p_csr_assemble: term %d lives on another space", t);
-    if (coefs[t] == 0.0) continue;
-    for (int j = 0; j < A->P; j++)
-    {
-      B2P_LAUNCH(set_unit_kernel, blocks(nE, 256), 256, 0, s, A->d_x, nE, A->P, j);
-      B2P_CUDA(ctx, cudaMemsetAsync(A->d_y, 0, sizeof(double) * nE, s));
-      ApplyRange rg;
-      rg.n_owned = nE;  // the whole E-vector is "owned": no ghost segment (nE >= the operator's L-size)
-      int rc = apply_range(op, A->d_eidx, 1.0, A->d_x, A->d_y, rg, 0, s);
-      if (rc) return rc;
-      B2P_LAUNCH(scatter_column_kernel, blocks(nE, 256), 256, 0, s, A->d_y, A->d_pos, A->d_gidx, nE, A->P, A->PS, j, coefs[t], A->d_val);
-    }
-  }
-  B2P_CUDA(ctx, cudaGetLastError());
-  return B2P_SUCCESS;
+  return A ? csr_assemble_values(A, n_terms, ops, coefs, A->d_val, (cudaStream_t)stream) : B2P_ERR_ARG;
 }
 
 int64_t b2p_csr_rows(const b2p_csr *A) { return A ? A->n : -1; }
@@ -250,46 +416,17 @@ int b2p_csr_get_host(b2p_csr *A, int32_t *rowptr, int32_t *col, double *val, b2p
 
 int b2p_csr_eliminate(b2p_csr *A, const int32_t *ess_dofs, int64_t n_ess, int diag_policy, b2p_stream stream)
 {
-  if (!A || (n_ess > 0 && !ess_dofs)) return B2P_ERR_ARG;
-  if (n_ess <= 0) return B2P_SUCCESS;
-  b2p_ctx *ctx = A->ctx;
-  cudaStream_t s = (cudaStream_t)stream;
-  for (int64_t i = 0; i < n_ess; i++)
-    B2P_CHECK(ctx, ess_dofs[i] >= 0 && ess_dofs[i] < A->n, B2P_ERR_ARG, "b2p_csr_eliminate: essential dof %d outside the matrix", ess_dofs[i]);
-  int32_t *d_ess = nullptr;
-  char *d_flag = nullptr;
-  int rc = upload(ctx, ess_dofs, (size_t)n_ess, &d_ess);
-  if (rc) return rc;
-  if (cudaMalloc(&d_flag, (size_t)A->n) != cudaSuccess)
-  {
-    cudaFree(d_ess);
-    set_error(ctx, "b2p_csr_eliminate: out of device memory");
-    return B2P_ERR_CUDA;
-  }
-  cudaMemsetAsync(d_flag, 0, (size_t)A->n, s);
-  B2P_LAUNCH(mark_kernel, blocks(n_ess, 256), 256, 0, s, d_ess, n_ess, d_flag);
-  B2P_LAUNCH(csr_eliminate_kernel, blocks(A->n, 256), 256, 0, s, A->n, A->d_rowptr, A->d_col, A->d_val, d_flag, diag_policy == 1 ? 1 : 0);
-  cudaStreamSynchronize(s);
-  cudaFree(d_ess);
-  cudaFree(d_flag);
-  B2P_CUDA(ctx, cudaGetLastError());
-  return B2P_SUCCESS;
+  return A ? csr_eliminate_values(A, ess_dofs, n_ess, diag_policy, A->d_val, (cudaStream_t)stream) : B2P_ERR_ARG;
 }
 
 int b2p_csr_mult(b2p_csr *A, const double *x, double *y, b2p_stream stream)
 {
-  if (!A || !x || !y) return B2P_ERR_ARG;
-  B2P_LAUNCH(csr_mult_kernel, blocks(A->n * CSR_LANES, 256), 256, 0, (cudaStream_t)stream, A->n, A->d_rowptr, A->d_col, A->d_val, x, y);
-  B2P_CUDA(A->ctx, cudaGetLastError());
-  return B2P_SUCCESS;
+  return A ? csr_mult_values(A, A->d_val, x, y, (cudaStream_t)stream) : B2P_ERR_ARG;
 }
 
 int b2p_csr_diag(b2p_csr *A, double *d, b2p_stream stream)
 {
-  if (!A || !d) return B2P_ERR_ARG;
-  B2P_LAUNCH(csr_diag_kernel, blocks(A->n, 256), 256, 0, (cudaStream_t)stream, A->n, A->d_rowptr, A->d_col, A->d_val, d);
-  B2P_CUDA(A->ctx, cudaGetLastError());
-  return B2P_SUCCESS;
+  return A ? csr_diag_values(A, A->d_val, d, (cudaStream_t)stream) : B2P_ERR_ARG;
 }
 
 void b2p_csr_destroy(b2p_csr *A)

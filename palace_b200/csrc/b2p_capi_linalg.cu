@@ -22,6 +22,7 @@ struct b2p_solver
 namespace b2p
 {
 Solver *solver_of(b2p_solver *s) { return s ? s->s.get() : nullptr; }
+std::unique_ptr<Solver> take_solver(b2p_solver *s) { return s ? std::move(s->s) : nullptr; }
 Operator *operator_of(b2p_operator *A) { return A ? A->op.get() : nullptr; }
 b2p_operator *wrap_operator(std::unique_ptr<Operator> &&op)  // (handles of operators built in other translation units)
 {

@@ -520,6 +520,48 @@ public:
   }
   const int32_t *EssentialTrueDofs() const override { return d_ess; }
   int64_t NumEssential() const override { return n_ess; }
+  // Full assembly of both parts into vr / vi [nnz] on a pattern built from PatternOp() (b2p_csr_create): from the fused sums
+  // S_re and S_im when they exist (dense or block terms: P launches each), else term by term with the real and then the
+  // imaginary coefficients. Essential rows as in ComplexParOperator (rap.cpp:481-517): Ar with the operator's diagonal policy,
+  // Ai with DIAG_ZERO.
+  b2p_op *PatternOp() const { return terms[0].op; }
+  bool HasReal() const
+  {
+    for (auto &t : terms)
+      if (t.cr != 0.0) return true;
+    return false;
+  }
+  int AssembleValues(b2p_csr *A, double *vr, double *vi) const
+  {
+    cudaStream_t s = ctx->stream;
+    int rc;
+    if (sum_re)
+    {
+      const double one = 1.0;
+      rc = csr_assemble_values(A, 1, &sum_re, &one, vr, s);
+      if (!rc) rc = csr_assemble_values(A, 1, &sum_im, &one, vi, s);
+    }
+    else
+    {
+      std::vector<b2p_op *> ops;
+      std::vector<double> cr, ci;
+      for (auto &t : terms)
+      {
+        ops.push_back(t.op);
+        cr.push_back(t.cr);
+        ci.push_back(t.ci);
+      }
+      rc = csr_assemble_values(A, (int)ops.size(), ops.data(), cr.data(), vr, s);
+      if (!rc) rc = csr_assemble_values(A, (int)ops.size(), ops.data(), ci.data(), vi, s);
+    }
+    if (rc || n_ess <= 0) return rc;
+    std::vector<int32_t> ess((size_t)n_ess);
+    B2P_CUDA(ctx, cudaMemcpyAsync(ess.data(), d_ess, sizeof(int32_t) * n_ess, cudaMemcpyDeviceToHost, s));
+    B2P_CUDA(ctx, cudaStreamSynchronize(s));
+    rc = csr_eliminate_values(A, ess.data(), n_ess, diag_policy, vr, s);
+    if (!rc) rc = csr_eliminate_values(A, ess.data(), n_ess, 0, vi, s);
+    return rc;
+  }
   void Mult(CCPtr x, CPtr y) const override { apply(x, y, false); }
   void MultHermitianTranspose(CCPtr x, CPtr y) const override { apply(x, y, true); }
   void AssembleDiagonal(CPtr d) const override
@@ -569,6 +611,8 @@ class ComplexWrapperOperator : public ComplexOperator
 
 public:
   ComplexWrapperOperator(b2p_ctx *c, const Operator *ar, const Operator *ai) : ComplexOperator(c, (ar ? ar : ai)->Height()), Ar(ar), Ai(ai) {}
+  const Operator *Real() const { return Ar; }
+  const Operator *Imag() const { return Ai; }
   void apply(CCPtr x, CPtr y, bool herm) const
   {
     const double si = herm ? -1.0 : 1.0;  // A^H = Ar^T - i Ai^T
@@ -945,6 +989,248 @@ public:
 
 namespace
 {
+// The real matrices a complex coarse solver hands its inner solver. Both are non-symmetric in general (Floquet terms, the
+// sum Ar + Ai): only Mult and the diagonal are provided.
+class CsrValuesOperator : public Operator
+{
+  b2p_csr *A;
+  const double *val;
+
+public:
+  CsrValuesOperator(b2p_ctx *c, b2p_csr *a, const double *v) : Operator(c, b2p_csr_rows(a), b2p_csr_rows(a)), A(a), val(v) {}
+  void Mult(const double *x, double *y) const override { csr_mult_values(A, val, x, y, ctx->stream); }
+  void MultTranspose(const double *, double *) const override { set_error(ctx, "assembled complex coarse matrix: no transpose"); }
+  void AssembleDiagonal(double *d) const override { csr_diag_values(A, val, d, ctx->stream); }
+};
+class CsrBlock2Operator : public Operator
+{
+  b2p_csr *A;
+  const double *vr, *vi;
+
+public:
+  CsrBlock2Operator(b2p_ctx *c, b2p_csr *a, const double *r, const double *i)
+    : Operator(c, 2 * b2p_csr_rows(a), 2 * b2p_csr_rows(a)), A(a), vr(r), vi(i)
+  {
+  }
+  void Mult(const double *x, double *y) const override { csr_block2_mult(A, vr, vi, x, y, ctx->stream); }
+  void MultTranspose(const double *, double *) const override { set_error(ctx, "assembled complex coarse matrix: no transpose"); }
+  void AssembleDiagonal(double *d) const override { csr_block2_diag(A, vr, d, ctx->stream); }
+};
+}  // namespace
+
+// MfemWrapperSolver<ComplexOperator> (linalg/solver.cpp:33-177) on the device: SetOperator assembles both parts of the complex
+// operator on one CSR pattern and hands a REAL matrix to the inner solver (and its preconditioner):
+//   * default: Ar + Ai; Mult applies the real solver to the real and the imaginary part separately;
+//   * complex_matrix: the 2n block [[Ar, Ai], [Ai, -Ar]] (applied by csr_block2_mult, never formed), solved once for
+//     [xr; -xi] with the right-hand side [br; bi].
+// A part that is absent (no real / no imaginary coefficient, or a NULL part of a wrapped operator) leaves the other part alone
+// as the matrix. The symbolic phase runs once per operator: a later SetOperator with the same operator (new coefficients)
+// only re-assembles the values.
+class ComplexAssembledSolver : public ComplexSolver
+{
+  enum Form { NONE, REAL, IMAG, SUM, BLOCK };
+  std::unique_ptr<Solver> inner, pc;
+  bool complex_matrix;
+  const ComplexOperator *src = nullptr;  // the operator whose pattern `csr` holds
+  const b2p_op *src_pattern = nullptr;
+  b2p_csr *csr = nullptr;
+  DVec vr, vi, vsum;
+  Form form = NONE;
+  std::unique_ptr<Operator> Ac;
+  int32_t *d_rp2 = nullptr, *d_col2 = nullptr;  // explicit block matrix (on request)
+  DVec v2;
+  bool v2_current = false;
+  int64_t n = 0;
+  mutable DVec X, Y;
+
+  void release_pattern()
+  {
+    b2p_csr_destroy(csr);
+    csr = nullptr;
+    cudaFree(d_rp2);
+    cudaFree(d_col2);
+    d_rp2 = d_col2 = nullptr;
+    src = nullptr;
+    src_pattern = nullptr;
+  }
+
+public:
+  ComplexAssembledSolver(b2p_ctx *c, std::unique_ptr<Solver> &&in, std::unique_ptr<Solver> &&p, bool cm)
+    : ComplexSolver(c), inner(std::move(in)), pc(std::move(p)), complex_matrix(cm)
+  {
+  }
+  ~ComplexAssembledSolver() override { release_pattern(); }
+  bool SetOperator(const ComplexOperator &op) override
+  {
+    const auto *par = dynamic_cast<const ComplexParOperator *>(&op);
+    const auto *wrap = dynamic_cast<const ComplexWrapperOperator *>(&op);
+    const ParOperator *pr = nullptr, *pi = nullptr;
+    bool has_re, has_im;
+    b2p_op *pattern;
+    if (par)
+    {
+      has_re = par->HasReal();
+      has_im = !par->IsReal();
+      pattern = par->PatternOp();
+    }
+    else if (wrap)
+    {
+      pr = dynamic_cast<const ParOperator *>(wrap->Real());
+      pi = dynamic_cast<const ParOperator *>(wrap->Imag());
+      if ((wrap->Real() && !pr) || (wrap->Imag() && !pi))
+      {
+        set_error(ctx, "b2p_csolver_assembled: the parts of a wrapped complex operator must be ParOperators (b2p_operator_par) to be assembled");
+        return false;
+      }
+      has_re = pr != nullptr;
+      has_im = pi != nullptr;
+      pattern = (pr ? pr : pi)->PatternOp();
+      if (pr && pi)
+      {
+        const b2p_op *a = pr->PatternOp(), *b = pi->PatternOp();
+        bool same = a->ne == b->ne && a->P == b->P && a->PS == b->PS && a->lsize == b->lsize;
+        if (same && a->lidx != b->lidx)
+        {
+          std::vector<int32_t> ha((size_t)a->ne * a->PS), hb(ha.size());
+          same = cudaMemcpy(ha.data(), a->lidx, ha.size() * sizeof(int32_t), cudaMemcpyDeviceToHost) == cudaSuccess &&
+                 cudaMemcpy(hb.data(), b->lidx, hb.size() * sizeof(int32_t), cudaMemcpyDeviceToHost) == cudaSuccess && ha == hb;
+        }
+        if (!same)
+        {
+          set_error(ctx, "b2p_csolver_assembled: the real and imaginary parts live on different spaces");
+          return false;
+        }
+      }
+    }
+    else
+    {
+      set_error(ctx, "b2p_csolver_assembled must be able to assemble its operator: b2p_coperator_par, or b2p_coperator_wrap of b2p_operator_par parts");
+      return false;
+    }
+    if (!has_re && !has_im)
+    {
+      set_error(ctx, "Empty ComplexOperator for b2p_csolver_assembled!");
+      return false;
+    }
+    if (src != &op || src_pattern != pattern || !csr)
+    {
+      release_pattern();
+      if (b2p_csr_create(ctx, pattern, &csr) != B2P_SUCCESS) return false;
+      src = &op;
+      src_pattern = pattern;
+    }
+    const int64_t nnz = b2p_csr_nnz(csr);
+    if (vr.n != nnz) vr.resize(ctx, std::max<int64_t>(nnz, 1));
+    if (vi.n != nnz) vi.resize(ctx, std::max<int64_t>(nnz, 1));
+    int rc = B2P_SUCCESS;
+    if (par)
+      rc = par->AssembleValues(csr, vr.p, vi.p);
+    else
+    {
+      if (pr) rc = pr->AssembleValues(csr, vr.p);
+      if (!rc && pi) rc = pi->AssembleValues(csr, vi.p);
+    }
+    if (rc)
+    {
+      release_pattern();
+      form = NONE;
+      Ac.reset();
+      return false;
+    }
+    n = b2p_csr_rows(csr);
+    if (has_re && has_im && complex_matrix)
+    {
+      form = BLOCK;
+      Ac = std::make_unique<CsrBlock2Operator>(ctx, csr, vr.p, vi.p);
+    }
+    else if (has_re && has_im)
+    {
+      form = SUM;
+      if (vsum.n != vr.n) vsum.resize(ctx, vr.n);
+      vec::axpbypcz(ctx, 1.0, vr.p, 1.0, vi.p, 0.0, vsum.p, nnz);
+      Ac = std::make_unique<CsrValuesOperator>(ctx, csr, vsum.p);
+    }
+    else
+    {
+      form = has_re ? REAL : IMAG;
+      Ac = std::make_unique<CsrValuesOperator>(ctx, csr, has_re ? vr.p : vi.p);
+    }
+    v2_current = false;
+    if (pc) pc->SetOperator(*Ac);
+    inner->SetOperator(*Ac);
+    return true;
+  }
+  void Mult(CCPtr x, CPtr y) const override
+  {
+    if (form == NONE)
+    {
+      set_error(ctx, "b2p_csolver_assembled: applied without an assembled operator");
+      return;
+    }
+    inner->SetInitialGuess(initial_guess);
+    if (form != BLOCK)
+    {
+      inner->Mult(x.re, y.re);
+      inner->Mult(x.im, y.im);
+      return;
+    }
+    // A [yr; -yi] = [xr; xi]  (solver.cpp:158-176)
+    if (X.n != 2 * n) X.resize(ctx, 2 * n);
+    if (Y.n != 2 * n) Y.resize(ctx, 2 * n);
+    vec::copy(ctx, X.p, x.re, n);
+    vec::copy(ctx, X.p + n, x.im, n);
+    if (initial_guess)
+    {
+      vec::copy(ctx, Y.p, y.re, n);
+      vec::axpby(ctx, -1.0, y.im, 0.0, Y.p + n, n);
+    }
+    inner->Mult(X.p, Y.p);
+    vec::copy(ctx, y.re, Y.p, n);
+    vec::axpby(ctx, -1.0, Y.p + n, 0.0, y.im, n);
+  }
+  // entries of the real matrix the inner solver sees (4 nnz for the block form)
+  int64_t Nnz() const { return form == NONE ? -1 : (form == BLOCK ? 4 : 1) * b2p_csr_nnz(csr); }
+  // CSR arrays of that matrix (device, owned here); the block form is built on the first request and refilled after a new
+  // assembly.
+  int DeviceArrays(int64_t *rows, int64_t *nnz, const int32_t **rowptr, const int32_t **col, const double **val)
+  {
+    B2P_CHECK(ctx, form != NONE, B2P_ERR_ARG, "b2p_csolver_assembled_device_arrays before set_operator");
+    const int32_t *rp, *cl;
+    const double *v = nullptr;
+    if (form == BLOCK)
+    {
+      if (!d_rp2)
+      {
+        int rc = csr_block2_pattern(csr, &d_rp2, &d_col2);
+        if (rc) return rc;
+      }
+      if (v2.n != 4 * b2p_csr_nnz(csr)) v2.resize(ctx, std::max<int64_t>(4 * b2p_csr_nnz(csr), 1));
+      if (!v2_current)
+      {
+        int rc = csr_block2_fill(csr, vr.p, vi.p, v2.p, ctx->stream);
+        if (rc) return rc;
+        v2_current = true;
+      }
+      rp = d_rp2;
+      cl = d_col2;
+      v = v2.p;
+    }
+    else
+    {
+      b2p_csr_device_arrays(csr, &rp, &cl, nullptr);
+      v = form == SUM ? vsum.p : (form == REAL ? vr.p : vi.p);
+    }
+    if (rows) *rows = (form == BLOCK ? 2 : 1) * n;
+    if (nnz) *nnz = Nnz();
+    if (rowptr) *rowptr = rp;
+    if (col) *col = cl;
+    if (val) *val = v;
+    return B2P_SUCCESS;
+  }
+};
+
+namespace
+{
 inline void ApplyPlaneRotation(cplx &dx, cplx &dy, const double cs, const cplx sn)
 {
   const cplx t = cs * dx + sn * dy;
@@ -1256,6 +1542,7 @@ struct b2p_solver;
 namespace b2p
 {
 Solver *solver_of(b2p_solver *s);
+std::unique_ptr<Solver> take_solver(b2p_solver *s);
 Operator *operator_of(b2p_operator *A);
 }
 
@@ -1372,6 +1659,39 @@ int b2p_csolver_real_pc(b2p_ctx *ctx, b2p_solver *real_pc, b2p_csolver **out)
   h->s = std::make_unique<RealPcSolver>(ctx, solver_of(real_pc));
   *out = h;
   return B2P_SUCCESS;
+}
+int b2p_csolver_assembled(b2p_ctx *ctx, b2p_solver *inner, b2p_solver *inner_pc, int complex_matrix, b2p_csolver **out)
+{
+  B2P_CHECK(ctx, ctx && inner && solver_of(inner) && out, B2P_ERR_ARG, "b2p_csolver_assembled: bad argument");
+  auto *k = dynamic_cast<IterativeSolver *>(solver_of(inner));
+  if (inner_pc)
+  {
+    B2P_CHECK(ctx, solver_of(inner_pc) && k, B2P_ERR_ARG, "b2p_csolver_assembled: a preconditioner needs a Krylov inner solver");
+    k->SetPreconditioner(solver_of(inner_pc));
+  }
+  auto *h = new b2p_csolver;
+  h->s = std::make_unique<ComplexAssembledSolver>(ctx, take_solver(inner), take_solver(inner_pc), complex_matrix != 0);
+  *out = h;
+  return B2P_SUCCESS;
+}
+// the assembled solver itself, or the one a complex multigrid took over as its coarse solver
+static ComplexAssembledSolver *assembled_of(b2p_csolver *s)
+{
+  ComplexSolver *p = s ? s->s.get() : nullptr;
+  if (auto *g = dynamic_cast<ComplexGeometricMultigridSolver *>(p)) p = g->B[0].get();
+  return dynamic_cast<ComplexAssembledSolver *>(p);
+}
+int64_t b2p_csolver_assembled_nnz(b2p_csolver *s)
+{
+  auto *a = assembled_of(s);
+  return a ? a->Nnz() : -1;
+}
+int b2p_csolver_assembled_device_arrays(b2p_csolver *s, int64_t *rows, int64_t *nnz, const int32_t **rowptr, const int32_t **col,
+                                        const double **val)
+{
+  auto *a = assembled_of(s);
+  if (!a) return B2P_ERR_ARG;
+  return a->DeviceArrays(rows, nnz, rowptr, col, val);
 }
 int b2p_csolver_jacobi(b2p_ctx *ctx, double omega, b2p_csolver **out)
 {

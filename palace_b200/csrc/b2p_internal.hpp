@@ -237,4 +237,17 @@ int launch_dense_apply(b2p_op *op, const int32_t *lidx, double alpha, const doub
 int launch_dense_diag(b2p_op *op, double *diag, cudaStream_t s);
 int launch_geom_hex(b2p_ctx *ctx, int ne, int k, int q1d, const double *d_xe, const double *d_B, const double *d_G,
                     const double *d_qw, double *d_qd, cudaStream_t s);
+// CSR assembly on value arrays other than the handle's own (b2p_assemble.cu): the complex coarse solver keeps the real and
+// imaginary parts of one operator as two value arrays [nnz] on ONE pattern.
+double *csr_values(b2p_csr *A);
+int csr_assemble_values(b2p_csr *A, int n_terms, b2p_op *const *ops, const double *coefs, double *val, cudaStream_t s);
+int csr_eliminate_values(b2p_csr *A, const int32_t *ess_dofs, int64_t n_ess, int diag_policy, double *val, cudaStream_t s);
+int csr_mult_values(b2p_csr *A, const double *val, const double *x, double *y, cudaStream_t s);
+int csr_diag_values(b2p_csr *A, const double *val, double *d, cudaStream_t s);
+// The real 2n form [[Ar, Ai], [Ai, -Ar]] of Ar + i Ai (values vr, vi on A's pattern): y = B x and d = diag(B) = [diag Ar; -diag Ar]
+// without forming B; csr_block2_pattern (host, device arrays owned by the caller) and csr_block2_fill form it explicitly.
+int csr_block2_mult(b2p_csr *A, const double *vr, const double *vi, const double *x, double *y, cudaStream_t s);
+int csr_block2_diag(b2p_csr *A, const double *vr, double *d, cudaStream_t s);
+int csr_block2_pattern(b2p_csr *A, int32_t **rowptr2, int32_t **col2);
+int csr_block2_fill(b2p_csr *A, const double *vr, const double *vi, double *val2, cudaStream_t s);
 }  // namespace b2p

@@ -165,6 +165,10 @@ public:
   // The eliminated sum as one device CSR matrix (ParOperator::ParallelAssemble, rap.cpp:84-152; coarse levels, single
   // partition); the caller owns the result (b2p_csr_destroy). Throws through set_error + nullptr on failure.
   b2p_csr *FullAssemble() const;
+  // The numeric phase of FullAssemble into `val` (nnz entries on a pattern built from PatternOp()): the complex coarse solver
+  // re-assembles the parts of a ComplexWrapperOperator without a new symbolic phase.
+  int AssembleValues(b2p_csr *A, double *val) const;
+  b2p_op *PatternOp() const { return terms[0].op; }
   const int32_t *EssentialTrueDofs() const override { return d_ess; }
   int64_t NumEssential() const override { return n_ess; }
   int64_t lsize;

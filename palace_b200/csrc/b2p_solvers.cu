@@ -333,6 +333,20 @@ b2p_csr *ParOperator::FullAssemble() const
   }
   b2p_csr *A = nullptr;
   if (b2p_csr_create(ctx, terms[0].op, &A) != B2P_SUCCESS) return nullptr;
+  if (AssembleValues(A, csr_values(A)) != B2P_SUCCESS)
+  {
+    b2p_csr_destroy(A);
+    return nullptr;
+  }
+  return A;
+}
+int ParOperator::AssembleValues(b2p_csr *A, double *val) const
+{
+  if (halo && halo->n_ghost > 0)
+  {
+    set_error(ctx, "ParOperator::FullAssemble: partitioned spaces are not assembled (the coarse matrix lives on one device)");
+    return B2P_ERR_UNSUPPORTED;
+  }
   std::vector<b2p_op *> ops;
   std::vector<double> cf;
   for (auto &t : terms)
@@ -346,13 +360,9 @@ b2p_csr *ParOperator::FullAssemble() const
     cudaMemcpyAsync(ess.data(), d_ess, sizeof(int32_t) * n_ess, cudaMemcpyDeviceToHost, ctx->stream);
     cudaStreamSynchronize(ctx->stream);
   }
-  if (b2p_csr_assemble(A, (int)ops.size(), ops.data(), cf.data(), (b2p_stream)ctx->stream) != B2P_SUCCESS ||
-      b2p_csr_eliminate(A, ess.data(), n_ess, diag_policy, (b2p_stream)ctx->stream) != B2P_SUCCESS)
-  {
-    b2p_csr_destroy(A);
-    return nullptr;
-  }
-  return A;
+  int rc = csr_assemble_values(A, (int)ops.size(), ops.data(), cf.data(), val, ctx->stream);
+  if (!rc) rc = csr_eliminate_values(A, ess.data(), n_ess, diag_policy, val, ctx->stream);
+  return rc;
 }
 void ParOperator::AssembleDiagonal(double *d) const
 {
