@@ -456,6 +456,10 @@ int b2p_coperator_assemble_diagonal(b2p_coperator *A, double *dr, double *di);
  * operator: the smoothers / solvers that hold A see the new matrix at their next SetOperator. */
 int b2p_coperator_set_coefficients(b2p_coperator *A, int n_terms, const double *coef_re, const double *coef_im);
 long b2p_coperator_fused_applies(b2p_coperator *A);
+/* Route of a b2p_coperator_par's Mult / MultHermitianTranspose / AddMult: 0 term by term (2-4 real applies per term), 1 two real
+ * sums S_re and S_im (4 applies), 2 one pass over the geometry on the nd4 kernel (p <= 3), 3 one pass on the CTA-per-batch
+ * kernel (symmetric kinds at p = 4 ... 6, block sums at p = 2 ... 6); -1 if A is not a sum operator. */
+int b2p_coperator_fused_path(b2p_coperator *A);
 void b2p_coperator_destroy(b2p_coperator *A);
 /* A real preconditioner (any b2p_solver, e.g. the multigrid) applied to the real and imaginary parts: the
  * "PCMatReal" configuration (models/spaceoperator.cpp:1098-1105, utils/configfile.hpp:1051). */

@@ -773,6 +773,10 @@ class ComplexOperator:
         f.restype = C.c_long
         return int(f(self.h))
 
+    def fused_path(self):
+        """0 term by term, 1 two real sums, 2 one pass (nd4, p <= 3), 3 one pass (CTA-per-batch kernel)."""
+        return int(lib().b2p_coperator_fused_path(self.h))
+
     def mult_hermitian_transpose(self, xr, xi, yr, yi):
         _chk(lib().b2p_coperator_mult_hermitian_transpose(self.h, _vp(xr), _vp(xi), _vp(yr), _vp(yi)), self.ctx.h)
 

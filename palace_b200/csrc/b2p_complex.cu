@@ -332,17 +332,27 @@ public:
       }
       if (b2p_op_create_sum(ctx, (int)ops.size(), ops.data(), cr.data(), &sum_re) == B2P_SUCCESS &&
           b2p_op_create_sum(ctx, (int)ops.size(), ops.data(), ci.data(), &sum_im) == B2P_SUCCESS)
+      {
+        // Block sums at q1d = p + 1 with mirror-symmetric tables: one nd_hex_apply7_kernel<..., CPLX> launch reads S_re's and
+        // S_im's coefficient blocks (bcoef, or bcoef_t for the Hermitian transpose) instead of 4 applies. S_re / S_im stay:
+        // assembly (AssembleValues) reads them, and p = 1 and other tables keep the 4 applies.
+        cta = block && !sum_re->dense && sum_re->bcoef && sum_im->bcoef && nd_hex_apply7_eligible(sum_re);
+        fused_imag = !IsReal();
         return;
+      }
       if (sum_re) b2p_op_destroy(sum_re);
       if (sum_im) b2p_op_destroy(sum_im);
       sum_re = sum_im = nullptr;  // not fusable (mixed kinds / spaces): term by term
       return;
     }
+    // p <= 3: nd_hex_apply4_kernel<..., CPLX>; p = 4 ... 6: nd_hex_apply7_kernel<..., CPLX> for sums of two or more terms (a
+    // single term keeps its real applies)
+    const bool cta7 = o0->p >= 4 && terms.size() >= 2;
     for (auto &t : terms)
     {
-      const b2p_op *o = t.op;
-      if (!nd_hex_apply4z_eligible(o) || o->bcoef || o->geom != o0->geom || o->p != o0->p || o->q1d != o0->q1d || o->ne != o0->ne ||
-          o->lsize != o0->lsize || o->PS != o0->PS || !o->ecoef || !o->lidx_bc)
+      b2p_op *o = t.op;
+      if (!(cta7 ? nd_hex_apply7_eligible(o) : nd_hex_apply4z_eligible(o)) || o->bcoef || o->geom != o0->geom || o->p != o0->p ||
+          o->q1d != o0->q1d || o->ne != o0->ne || o->lsize != o0->lsize || o->PS != o0->PS || !o->ecoef || !o->lidx_bc)
         return;
     }
     const size_t nidx = (size_t)o0->ne * o0->PS;
@@ -359,6 +369,7 @@ public:
       if (cudaMemcpy(fused_e18[i].data(), terms[i].op->ecoef, fused_e18[i].size() * sizeof(double), cudaMemcpyDeviceToHost) != cudaSuccess)
         return;
     fused = fill_fused();
+    cta = fused && cta7;
   }
 
   // zcoef / zcoef_h from the cached per-term material tensors and the current scalar coefficients
@@ -417,15 +428,23 @@ public:
       terms[t].cr = cr[t];
       terms[t].ci = ci[t];
     }
-    if (fused) fused = fill_fused();
+    if (fused)
+    {
+      fused = fill_fused();
+      cta = cta && fused;
+    }
     if (sum_re)
     {
       std::vector<b2p_op *> ops;
       for (auto &t : terms) ops.push_back(t.op);
       b2p_op_sum_set_coefficients(sum_re, (int)ops.size(), ops.data(), cr);
       b2p_op_sum_set_coefficients(sum_im, (int)ops.size(), ops.data(), ci);
+      fused_imag = !IsReal();
     }
   }
+  // b2p_coperator_fused_path: 0 term by term, 1 two real sums, 2 one pass on nd_hex_apply4_kernel, 3 one pass on
+  // nd_hex_apply7_kernel
+  int FusedPath() const { return cta ? 3 : fused ? 2 : sum_re ? 1 : 0; }
 
   // operator.cpp:98-134 with A = sum_i c_i A_i: y_r = sum (c^r A x_r - c^i A x_i), y_i = sum (c^i A x_r + c^r A x_i);
   // essential rows as in ComplexParOperator::Mult (rap.cpp:481-517)
@@ -453,7 +472,21 @@ public:
   {
     cudaStream_t s = ctx->stream;
     b2p_op *o0 = terms[0].op;
-    if (fused && launch_nd_hex_apply4z(o0, fused_kind, o0->lidx_bc, herm ? zcoef_h : zcoef, fused_imag ? 1 : 0, alpha, x.re, x.im, y.re,
+    if (cta)
+    {
+      // one pass over the geometry for all terms and both parts; the Hermitian transpose conjugates the coupling (sgn = -1) and,
+      // for block sums, reads the transposed blocks
+      int rc;
+      if (sum_re)
+        rc = launch_nd_hex_apply7z(sum_re, B2P_ND_BLOCK, sum_re->lidx_bc, herm ? sum_re->bcoef_t : sum_re->bcoef,
+                                   herm ? sum_im->bcoef_t : sum_im->bcoef, fused_imag ? 1 : 0, herm ? -1.0 : 1.0, alpha, x.re, x.im,
+                                   y.re, y.im, s);
+      else
+        rc = launch_nd_hex_apply7z(o0, fused_kind, o0->lidx_bc, zcoef, nullptr, fused_imag ? 1 : 0, herm ? -1.0 : 1.0, alpha, x.re,
+                                   x.im, y.re, y.im, s);
+      if (rc == B2P_SUCCESS) n_fused_applies++;
+    }
+    else if (fused && launch_nd_hex_apply4z(o0, fused_kind, o0->lidx_bc, herm ? zcoef_h : zcoef, fused_imag ? 1 : 0, alpha, x.re, x.im, y.re,
                                        y.im, s) == B2P_SUCCESS)
       n_fused_applies++;
     else if (sum_re)
@@ -587,8 +620,8 @@ public:
 private:
   std::vector<Term> terms;
   int32_t *d_ess = nullptr;
-  // fused complex element operator (build_fused)
-  bool fused = false, fused_imag = false;
+  // fused complex element operator (build_fused); cta: its applies (or the block sums') run on nd_hex_apply7_kernel<..., CPLX>
+  bool fused = false, fused_imag = false, cta = false;
   // the real and imaginary coefficient sums as two operators: dense-basis terms, or hex terms with a mixed curl kind (block sums)
   b2p_op *sum_re = nullptr, *sum_im = nullptr;
   int fused_kind = 0;
@@ -1649,6 +1682,11 @@ long b2p_coperator_fused_applies(b2p_coperator *A)
 {
   auto *p = A ? dynamic_cast<ComplexParOperator *>(A->op.get()) : nullptr;
   return p ? p->n_fused_applies : -1;
+}
+int b2p_coperator_fused_path(b2p_coperator *A)
+{
+  auto *p = A ? dynamic_cast<ComplexParOperator *>(A->op.get()) : nullptr;
+  return p ? p->FusedPath() : -1;
 }
 void b2p_coperator_destroy(b2p_coperator *A) { delete A; }
 

@@ -1,6 +1,8 @@
 // High-order Nedelec hexahedron apply kernel: one CTA per element batch, one 1-D line per thread.
 //
 //   y_L += alpha * sum_e E_e^T  B^T  D  B  E_e x_L          (curl-curl, mass, curl-curl + mass),   p = 2 ... 6 at q1d = p + 1
+// and, in the CPLX instantiations, the complex sum  (y_r + i y_i) += alpha * sum_e E_e^T B^T (D_r + i D_i) B E_e (x_r + i x_i)
+// of a ComplexParOperator in one pass (both parts through the phases below, one after the other; DESIGN.md 4.3).
 //
 // Same operator as nd_hex_apply4_kernel. That kernel gives every WARP whole elements and keeps a (qy,qz) line of u, curl u
 // in registers through the pointwise D; at p >= 5 a lane then owns several lines (q1d^2 = 36, 49 > 32), the kernel spills
@@ -29,6 +31,7 @@
 // /root/reference/palace/fem/qfunctions/33/{hdiv,hcurl,hdivmass}_33_qf.h.
 #include <cmath>
 #include <cstdlib>
+#include <type_traits>
 
 #include "b2p_internal.hpp"
 #include "b2p_qf.cuh"
@@ -60,6 +63,20 @@ struct ND7Params
   double Gc[(P_ + 1) * (P_ + 1)];
 };
 
+// Complex apply (CPLX kernels): y_r + i y_i += alpha * E^T B^T (D_r + s i D_i) B E (x_r + i x_i), both parts in one pass.
+// ecoef: {mass Re, mass Im, curl Re, curl Im} 3x3 tensors per element (symmetric kinds) or the real four-tensor block
+// (B2P_ND_BLOCK, with ecoef_i the imaginary one); s = sgn (-1: Hermitian transpose, with the transposed blocks).
+template <int P_>
+struct ND7ParamsZ : ND7Params<P_>
+{
+  const double *xi, *ecoef_i;
+  double *yi;
+  double sgn;
+  int has_imag;  // some coefficient has an imaginary part (otherwise the parts never mix)
+};
+template <int P_, bool CPLX>
+using ND7ParamsT = std::conditional_t<CPLX, ND7ParamsZ<P_>, ND7Params<P_>>;
+
 // smallest row stride >= len that is = res modulo 16 words (the 64-bit bank period of a half-warp)
 constexpr int nd7_stride(int len, int res)
 {
@@ -69,7 +86,7 @@ constexpr int nd7_stride(int len, int res)
 }
 constexpr int nd7_max(int a, int b) { return a > b ? a : b; }
 
-template <int P_, int KIND, int NE>
+template <int P_, int KIND, int NE, bool CPLX = false>
 struct ND7Layout
 {
   static constexpr int p = P_, q = P_ + 1, n = P_ + 1, QQ = q * q, Q = q * q * q, D3 = p * n * n, P = 3 * D3;
@@ -78,7 +95,9 @@ struct ND7Layout
   static constexpr bool BLOCK = (KIND == B2P_ND_BLOCK);
   static constexpr bool MASS = (KIND == B2P_ND_MASS || KIND == B2P_CURLCURL_MASS || BLOCK);
   static constexpr bool CURL = (KIND == B2P_CURLCURL || KIND == B2P_CURLCURL_MASS || BLOCK);
-  static constexpr int CE = BLOCK ? 36 : 18;  // coefficient doubles per element: two 3x3 tensors, four for the block form
+  // coefficient doubles per element and array: two 3x3 tensors, four for the block form and for the complex symmetric kinds
+  static constexpr int CEA = (BLOCK || CPLX) ? 36 : 18;
+  static constexpr int CE = (BLOCK && CPLX) ? 2 * CEA : CEA;  // complex block form: the imaginary block at + NE CEA
   static constexpr int LQ = NE * QQ;  // line slots of one component (all index extents padded to q)
   // Z -> Y arrays (region A), rows j: written by the Z phase at (j, i + q qz), read by the Y phase along j
   static constexpr int RS1 = nd7_stride(LQ, q);
@@ -92,8 +111,10 @@ struct ND7Layout
   static constexpr int B_X1 = 0, B_X2 = B_X1 + (MASS ? p * RS2 : 0), B_X3 = B_X2 + (CURL ? p * RS2 : 0),
                        B_Y1 = B_X3 + (CURL ? p * RS2 : 0), B_Y2 = B_Y1 + n * RS2, B_Z1 = B_Y2 + (CURL ? n * RS2 : 0),
                        B_Z3 = B_Z1 + n * RS2, SB = B_Z3 + (CURL ? n * RS2 : 0);
+  // CPLX: the point arrays of the real part (region P, same layout as at A_U), which the imaginary part's Z -> Y arrays would overwrite
+  static constexpr int OFF_P = SA + SB, SP = CPLX ? A_QP : 0;
   // GSM: q-data [NE][10][Q] and coefficient blocks [NE][CE] of the batch, staged by TMA bulk copies behind one mbarrier
-  static constexpr int GE = 10 * Q, OFF_G = (SA + SB + 1) & ~1, OFF_C = OFF_G + NE * GE, OFF_BAR = OFF_C + NE * CE;
+  static constexpr int GE = 10 * Q, OFF_G = (OFF_P + SP + 1) & ~1, OFF_C = OFF_G + NE * GE, OFF_BAR = OFF_C + NE * CE;
   static_assert(GE % 2 == 0, "16-byte blocks for the bulk copies");
   static constexpr int SMEM_BYTES_LDG = (SA + SB) * 8, SMEM_BYTES_GSM = (OFF_BAR + 2) * 8;
 };
@@ -123,14 +144,19 @@ __device__ __forceinline__ void scatter7(double *y, const VSplit &sp, double *si
 // belong to the same component's warps and its own work arrays) synchronise only that component's WPC warps (named barrier,
 // __syncwarp() for one warp) instead of the CTA; the components may drift apart by a phase. The other four hand-offs cross
 // components (X reads all three, the point arrays alias the Z -> Y arrays) and stay __syncthreads().
-template <int P_, int KIND, bool SPLIT, int NE, int WPC, int MINB, bool GSM, bool CBAR>
-__global__ void __launch_bounds__(3 * WPC * 32, MINB) nd_hex_apply7_kernel(const __grid_constant__ ND7Params<P_> prm)
+// CPLX: the batch's restriction, q-data and coefficient blocks are fetched once for both parts. Z, Y, X run for the real part
+// (into region P) and then the imaginary part; D forms the geometric transform once per point and couples the parts; Xt, Yt,
+// Zt + scatter run for the imaginary part (its point arrays alias the Z -> Y arrays) and then the real part.
+template <int P_, int KIND, bool SPLIT, int NE, int WPC, int MINB, bool GSM, bool CBAR, bool CPLX = false>
+__global__ void __launch_bounds__(3 * WPC * 32, MINB) nd_hex_apply7_kernel(const __grid_constant__ ND7ParamsT<P_, CPLX> prm)
 {
-  using L = ND7Layout<P_, KIND, NE>;
+  using L = ND7Layout<P_, KIND, NE, CPLX>;
   constexpr int p = L::p, q = L::q, n = L::n, QQ = L::QQ, Q = L::Q, D3 = L::D3, LQ = L::LQ, RS1 = L::RS1, RS2 = L::RS2;
   constexpr bool MASS = L::MASS, CURL = L::CURL;
   constexpr int NT = 3 * WPC * 32;
+  constexpr int NPART = CPLX ? 2 : 1;
   static_assert(LQ <= WPC * 32, "one line per thread");
+  static_assert(!CPLX || (GSM && !SPLIT), "complex apply: single partition, coefficients staged by TMA");
   constexpr int H = (q + 1) / 2;
 // table entry (row c, column i) through the stored half (indices are compile-time constants after unrolling)
 #define TBO(c, i) ((c) < H ? prm.Bo[(c) * p + (i)] : prm.Bo[(q - 1 - (c)) * p + (p - 1 - (i))])
@@ -224,7 +250,13 @@ __global__ void __launch_bounds__(3 * WPC * 32, MINB) nd_hex_apply7_kernel(const
     const int e0 = bb * NE, nel = min(NE, prm.ne - e0);
     mbar_expect_tx(bar_g, (uint32_t)(nel * (L::GE + L::CE) * sizeof(double)));
     tma_bulk_g2s_hint(sG, prm.qd + (size_t)e0 * L::GE, (uint32_t)(nel * L::GE * sizeof(double)), bar_g, once);
-    tma_bulk_g2s_hint(sC, prm.ecoef + (size_t)e0 * L::CE, (uint32_t)(nel * L::CE * sizeof(double)), bar_g, once);
+    if constexpr (CPLX && L::BLOCK)
+    {
+      tma_bulk_g2s_hint(sC, prm.ecoef + (size_t)e0 * L::CEA, (uint32_t)(nel * L::CEA * sizeof(double)), bar_g, once);
+      tma_bulk_g2s_hint(sC + NE * L::CEA, prm.ecoef_i + (size_t)e0 * L::CEA, (uint32_t)(nel * L::CEA * sizeof(double)), bar_g, once);
+    }
+    else
+      tma_bulk_g2s_hint(sC, prm.ecoef + (size_t)e0 * L::CE, (uint32_t)(nel * L::CE * sizeof(double)), bar_g, once);
   };
   uint32_t par_g = 0;
   if (GSM)
@@ -238,7 +270,15 @@ __global__ void __launch_bounds__(3 * WPC * 32, MINB) nd_hex_apply7_kernel(const
   }
 
   int32_t gi[n], ngi[n];
-  double xv[n];
+  double xv[n], xvi[n];  // gathered x (real part; CPLX: imaginary part, fetched behind the real part's Z phase)
+  auto load_xi = [&](const int32_t(&g)[n])
+  {
+    if constexpr (CPLX)
+    {
+#pragma unroll
+      for (int k = 0; k < n; k++) xvi[k] = g[k] == (int32_t)B2P_SKIP_IDX ? 0.0 : __ldg(prm.xi + (uint32_t)abs_idx(g[k]));
+    }
+  };
   load_idx(b, gi);
   ensure_ghosts(b);
   load_x(gi, xv);
@@ -252,12 +292,15 @@ __global__ void __launch_bounds__(3 * WPC * 32, MINB) nd_hex_apply7_kernel(const
     const bool has_next = bn < nb;
     const int e0 = b * NE, nel = min(NE, prm.ne - e0);
 
+#pragma unroll
+    for (int part = 0; part < NPART; part++)
+    {
     // ------------------------------------------------------------------ phase Z (contract k -> qz)
     if (zv)
     {
       double xs[n];
 #pragma unroll
-      for (int k = 0; k < n; k++) xs[k] = gi[k] < 0 ? -xv[k] : xv[k];
+      for (int k = 0; k < n; k++) xs[k] = gi[k] < 0 ? -((CPLX && part) ? xvi[k] : xv[k]) : ((CPLX && part) ? xvi[k] : xv[k]);
       double *oa = sA + sb * RS1 + se * QQ + sa;  // + q qz
       if (comp < 2)
       {
@@ -292,7 +335,8 @@ __global__ void __launch_bounds__(3 * WPC * 32, MINB) nd_hex_apply7_kernel(const
         }
       }
     }
-    if (has_next) load_idx(bn, ngi);
+    if (CPLX && part == 0) load_xi(gi);  // lands while the real part's Y and X run
+    if (has_next && part == 0) load_idx(bn, ngi);
     comp_sync();
 
     // ------------------------------------------------------------------ phase Y (contract j -> qy)
@@ -373,8 +417,9 @@ __global__ void __launch_bounds__(3 * WPC * 32, MINB) nd_hex_apply7_kernel(const
     //   curl_x = dy uz - dz uy = Bc (Z3 - Y2),  curl_y = dz ux - dx uz = Bo X3 - Gc Z1,  curl_z = dx uy - dy ux = Gc Y1 - Bo X2
     if (slot_ok)
     {
-      double *ou = sA + L::A_U + comp * q * LQ + tau;  // + qx LQ
-      double *oc = sA + L::A_C + comp * q * LQ + tau;
+      double *const sX = (CPLX && part == 0) ? sA + L::OFF_P : sA;  // point arrays of this part
+      double *ou = sX + L::A_U + comp * q * LQ + tau;  // + qx LQ
+      double *oc = sX + L::A_C + comp * q * LQ + tau;
       const double *in = sB + tau;  // + array + i RS2
       if (comp == 0)
       {
@@ -447,6 +492,7 @@ __global__ void __launch_bounds__(3 * WPC * 32, MINB) nd_hex_apply7_kernel(const
       }
     }
     __syncthreads();
+    }
     if (has_next)
     {
       ensure_ghosts(bn);
@@ -465,6 +511,78 @@ __global__ void __launch_bounds__(3 * WPC * 32, MINB) nd_hex_apply7_kernel(const
       const int qx = iota / LQ, t = iota % LQ, e = t / QQ, rr = t % QQ;
       if (e >= nel) continue;  // (tail slots hold zeros)
       const double *g = GSM ? sG + e * L::GE + qx * QQ + rr : prm.qd + (size_t)(e0 + e) * L::GE + qx * QQ + rr;
+      if constexpr (CPLX)
+      {
+        // t = A u (value), sc = Jd c (curl) for both parts; then per part  out_val = Cm t + Cx sc,  out_curl = Ck sc + Cw t with
+        // C = C_r on the own part and s C_i on the other (real part: - s C_i t_i, imaginary part: + s C_i t_r)
+        const double *Cr = sC + e * L::CEA;
+        const double *Ci = L::BLOCK ? Cr + NE * L::CEA : Cr + 9;  // symmetric kinds: {mass Re, mass Im, curl Re, curl Im}
+        constexpr int OK = L::BLOCK ? 9 : 18;                     // curl tensor
+        const double wdetJ = alpha * g[0];
+        double A[9], Jd[9], t[2][3], sc[2][3];
+#pragma unroll
+        for (int i = 0; i < 9; i++) A[i] = g[(1 + i) * Q];
+        if (CURL) cofactor33(A, Jd);
+        double *pp[2] = {sA + L::OFF_P + iota, sA + iota};
+#pragma unroll
+        for (int h = 0; h < 2; h++)
+        {
+          double u[3];
+#pragma unroll
+          for (int r3 = 0; r3 < 3; r3++) u[r3] = pp[h][L::A_U + r3 * NE * Q];
+          if (MASS) Ax33(A, u, t[h]);
+#pragma unroll
+          for (int r3 = 0; r3 < 3; r3++) u[r3] = pp[h][L::A_C + r3 * NE * Q];
+          if (CURL) Ax33(Jd, u, sc[h]);
+        }
+        // v += f (Cm t + Cx sc), w += f (Ck sc + Cw t)
+        auto couple = [&](const double *Cp, const double(&tt)[3], const double(&ss)[3], double f, double(&v)[3], double(&w)[3])
+        {
+          double a[3];
+          if (MASS)
+          {
+            Ax33(Cp, tt, a);
+#pragma unroll
+            for (int r = 0; r < 3; r++) v[r] += f * a[r];
+          }
+          if (CURL)
+          {
+            Ax33(Cp + OK, ss, a);
+#pragma unroll
+            for (int r = 0; r < 3; r++) w[r] += f * a[r];
+          }
+          if (L::BLOCK)
+          {
+            Ax33(Cp + 27, ss, a);
+#pragma unroll
+            for (int r = 0; r < 3; r++) v[r] += f * a[r];
+            Ax33(Cp + 18, tt, a);
+#pragma unroll
+            for (int r = 0; r < 3; r++) w[r] += f * a[r];
+          }
+        };
+        const double sg = prm.sgn;
+#pragma unroll
+        for (int h = 0; h < 2; h++)
+        {
+          double v[3] = {0.0, 0.0, 0.0}, w[3] = {0.0, 0.0, 0.0}, o[3];
+          couple(Cr, t[h], sc[h], 1.0, v, w);
+          if (prm.has_imag) couple(Ci, t[1 - h], sc[1 - h], h ? sg : -sg, v, w);
+          if (MASS)
+          {
+            Atx33(A, v, wdetJ, o);
+#pragma unroll
+            for (int r3 = 0; r3 < 3; r3++) pp[h][L::A_U + r3 * NE * Q] = o[r3];
+          }
+          if (CURL)
+          {
+            Atx33(Jd, w, wdetJ, o);
+#pragma unroll
+            for (int r3 = 0; r3 < 3; r3++) pp[h][L::A_C + r3 * NE * Q] = o[r3];
+          }
+        }
+        continue;
+      }
       const double *C = GSM ? sC + e * L::CE : prm.ecoef + (size_t)(e0 + e) * L::CE;
       double A[9], Cm[9], wdetJ, cm0, cc0;
       if (GSM)
@@ -558,12 +676,16 @@ __global__ void __launch_bounds__(3 * WPC * 32, MINB) nd_hex_apply7_kernel(const
       issue_geom(bn);
     }
 
+#pragma unroll
+    for (int part = NPART - 1; part >= 0; part--)
+    {
     // ------------------------------------------------------------------ phase Xt (transposed x-contraction)
     //   X1' = Bo^T w_x, X2' = -Bo^T cw_z, X3' = Bo^T cw_y ; Y1' = Bc^T w_y + Gc^T cw_z, Y2' = -Bc^T cw_x ;
     //   Z1' = Bc^T w_z - Gc^T cw_y, Z3' = Bc^T cw_x
     if (slot_ok)
     {
-      const double *wu = sA + L::A_U + tau, *wc = sA + L::A_C + tau;  // + (component q + qx) LQ
+      const double *const sX = (CPLX && part == 0) ? sA + L::OFF_P : sA;
+      const double *wu = sX + L::A_U + tau, *wc = sX + L::A_C + tau;  // + (component q + qx) LQ
       double *out = sB + tau;                                          // + array + i RS2
       if (comp == 0)
       {
@@ -708,6 +830,8 @@ __global__ void __launch_bounds__(3 * WPC * 32, MINB) nd_hex_apply7_kernel(const
     }
     if (zv)
     {
+      double *yp = prm.y;
+      if constexpr (CPLX) yp = part == 1 ? prm.yi : prm.y;
       const double *in = sA + sb * RS1 + se * QQ + sa;  // + array + q qz
       if (comp < 2)
       {
@@ -729,7 +853,7 @@ __global__ void __launch_bounds__(3 * WPC * 32, MINB) nd_hex_apply7_kernel(const
             v += TBC(qz, k) * a[qz];
             if (CURL) v += TGC(qz, k) * g[qz];
           }
-          scatter7<SPLIT>(prm.y, prm.sp, my_sink, gi[k], v);
+          scatter7<SPLIT>(yp, prm.sp, my_sink, gi[k], v);
         }
       }
       else
@@ -743,13 +867,17 @@ __global__ void __launch_bounds__(3 * WPC * 32, MINB) nd_hex_apply7_kernel(const
           double v = 0.0;
 #pragma unroll
           for (int qz = 0; qz < q; qz++) v += TBO(qz, k) * a[qz];
-          scatter7<SPLIT>(prm.y, prm.sp, my_sink, gi[k], v);
+          scatter7<SPLIT>(yp, prm.sp, my_sink, gi[k], v);
         }
       }
     }
+    if (part == 0)
+    {
 #pragma unroll
-    for (int k = 0; k < n; k++) gi[k] = ngi[k];
-    comp_sync();  // the next batch's Z phase overwrites the arrays Zt has just read
+      for (int k = 0; k < n; k++) gi[k] = ngi[k];
+    }
+    comp_sync();  // the next batch's Z phase (CPLX: the real part's Yt) overwrites the arrays Zt has just read
+    }
   }
 #undef TBO
 #undef TBC
@@ -759,37 +887,38 @@ __global__ void __launch_bounds__(3 * WPC * 32, MINB) nd_hex_apply7_kernel(const
 // Launch shape per order: elements per batch, warps per component, CTAs per SM (register cap 65536 / threads per SM), q-data
 // staged by TMA, component-wide barriers; chosen by A/B timing of the shapes (tools/nd7_ab.py, B2P_ND7_CFG). MINB_BLOCK is the
 // CTAs per SM of the B2P_ND_BLOCK instantiation, whose four-tensor D phase needs more registers than the cap of MINB allows at
-// p = 2, 3.
+// p = 2, 3. MINB_CPLX is that of the complex instantiations (both parts' gathered x live across the batch, and the D phase
+// holds both parts' values and curls), chosen so that none spills.
 template <int P_>
 struct ND7Shape;
 template <>
 struct ND7Shape<2>
 {
-  static constexpr int NE = 3, WPC = 1, MINB = 8, MINB_BLOCK = 4;  // 27 of 32 lanes, 96 threads
+  static constexpr int NE = 3, WPC = 1, MINB = 8, MINB_BLOCK = 4, MINB_CPLX = 4;  // 27 of 32 lanes, 96 threads
   static constexpr bool GSM = true, CBAR = true;
 };
 template <>
 struct ND7Shape<3>
 {
-  static constexpr int NE = 2, WPC = 1, MINB = 8, MINB_BLOCK = 5;  // 32 of 32 lanes, 96 threads
+  static constexpr int NE = 2, WPC = 1, MINB = 8, MINB_BLOCK = 5, MINB_CPLX = 4;  // 32 of 32 lanes, 96 threads
   static constexpr bool GSM = true, CBAR = true;
 };
 template <>
 struct ND7Shape<4>
 {
-  static constexpr int NE = 1, WPC = 1, MINB = 8, MINB_BLOCK = MINB;  // 25 of 32 lanes, 96 threads
+  static constexpr int NE = 1, WPC = 1, MINB = 8, MINB_BLOCK = MINB, MINB_CPLX = 4;  // 25 of 32 lanes, 96 threads
   static constexpr bool GSM = true, CBAR = true;
 };
 template <>
 struct ND7Shape<5>
 {
-  static constexpr int NE = 2, WPC = 3, MINB = 2, MINB_BLOCK = MINB;  // 72 of 96 lanes, 288 threads
+  static constexpr int NE = 2, WPC = 3, MINB = 2, MINB_BLOCK = MINB, MINB_CPLX = 1;  // 72 of 96 lanes, 288 threads
   static constexpr bool GSM = true, CBAR = true;
 };
 template <>
 struct ND7Shape<6>
 {
-  static constexpr int NE = 1, WPC = 2, MINB = 3, MINB_BLOCK = MINB;  // 49 of 64 lanes, 192 threads
+  static constexpr int NE = 1, WPC = 2, MINB = 3, MINB_BLOCK = MINB, MINB_CPLX = 2;  // 49 of 64 lanes, 192 threads
   static constexpr bool GSM = true, CBAR = true;
 };
 
@@ -841,6 +970,57 @@ int launch7_cfg(b2p_op *op, const int32_t *lidx, double alpha, const double *x, 
     B2P_LAUNCH_PDL(kern, grid, NT, shmem, s, prm);
   else
     B2P_LAUNCH(kern, grid, NT, shmem, s, prm);
+  B2P_CUDA(op->ctx, cudaGetLastError());
+  return B2P_SUCCESS;
+}
+
+// Complex apply: one launch for both parts (see ND7ParamsZ); `op` supplies geometry, restriction and tables.
+template <int P_, int KIND>
+int launch7z(b2p_op *op, const int32_t *lidx, const double *coef, const double *coef_i, int has_imag, double sgn, double alpha,
+             const double *xr, const double *xi, double *yr, double *yi, cudaStream_t s)
+{
+  using S = ND7Shape<P_>;
+  using L = ND7Layout<P_, KIND, S::NE, true>;
+  constexpr int NT = 3 * S::WPC * 32;
+  constexpr size_t shmem = L::SMEM_BYTES_GSM;
+  auto kern = nd_hex_apply7_kernel<P_, KIND, false, S::NE, S::WPC, S::MINB_CPLX, true, S::CBAR, true>;
+  static bool configured = false;
+  if (!configured)
+  {
+    B2P_CUDA(op->ctx, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)shmem));
+    configured = true;
+  }
+  if (op->ne <= 0) return B2P_SUCCESS;
+  ND7ParamsZ<P_> prm;
+  prm.lidx = lidx;
+  prm.qd = op->geom->qd;
+  prm.ecoef = coef;
+  prm.ecoef_i = coef_i;
+  prm.x = xr;
+  prm.xi = xi;
+  prm.y = yr;
+  prm.yi = yi;
+  prm.sink = op->ctx->d_sink;
+  prm.alpha = alpha;
+  prm.sgn = sgn;
+  prm.has_imag = has_imag;
+  prm.ne = op->ne;
+  prm.sp.n_owned = op->lsize;
+  prm.sp.xg = nullptr;
+  prm.sp.yg = nullptr;
+  prm.wait_flags = nullptr;
+  prm.wait_expect = nullptr;
+  prm.wait_n = 0;
+  prm.wait_from_elem = 0;
+  prm.iso = 0;
+  constexpr int q = P_ + 1, n = P_ + 1;
+  for (int i = 0; i < q * P_; i++) prm.Bo[i] = op->h_tab[i];
+  for (int i = 0; i < q * n; i++) prm.Bc[i] = op->h_tab[q * P_ + i];
+  for (int i = 0; i < q * n; i++) prm.Gc[i] = op->h_tab[q * P_ + q * n + i];
+  const int nb = (op->ne + S::NE - 1) / S::NE;
+  int grid = op->ctx->sm_count * S::MINB_CPLX;
+  if (grid > nb) grid = nb;
+  B2P_LAUNCH(kern, grid, NT, shmem, s, prm);
   B2P_CUDA(op->ctx, cudaGetLastError());
   return B2P_SUCCESS;
 }
@@ -930,6 +1110,32 @@ int launch_nd_hex_apply7(b2p_op *op, const int32_t *lidx, double alpha, const do
   B2P_CASE(6)
 #undef B2P_CASE
   set_error(op->ctx, "nd_hex_apply7: no kernel for p=%d q1d=%d kind=%d", op->p, op->q1d, op->kind);
+  return B2P_ERR_UNSUPPORTED;
+}
+
+int launch_nd_hex_apply7z(b2p_op *op, int kind, const int32_t *lidx, const double *coef, const double *coef_i, int has_imag, double sgn,
+                          double alpha, const double *xr, const double *xi, double *yr, double *yi, cudaStream_t s)
+{
+#define B2P_ZARGS op, lidx, coef, coef_i, has_imag, sgn, alpha, xr, xi, yr, yi, s
+  // block sums at p = 2 ... 6; symmetric kinds at p = 4, 5, 6 (p = 2, 3 run nd_hex_apply4_kernel<..., CPLX>)
+#define B2P_BLOCK(PP) \
+  if (op->p == PP && op->q1d == PP + 1 && kind == B2P_ND_BLOCK) return launch7z<PP, B2P_ND_BLOCK>(B2P_ZARGS);
+#define B2P_SYM(PP)                                                                     \
+  if (op->p == PP && op->q1d == PP + 1)                                                 \
+  {                                                                                     \
+    switch (kind)                                                                       \
+    {                                                                                   \
+      case B2P_CURLCURL: return launch7z<PP, B2P_CURLCURL>(B2P_ZARGS);                  \
+      case B2P_ND_MASS: return launch7z<PP, B2P_ND_MASS>(B2P_ZARGS);                    \
+      case B2P_CURLCURL_MASS: return launch7z<PP, B2P_CURLCURL_MASS>(B2P_ZARGS);        \
+    }                                                                                   \
+  }
+  B2P_BLOCK(2) B2P_BLOCK(3) B2P_BLOCK(4) B2P_BLOCK(5) B2P_BLOCK(6)
+  B2P_SYM(4) B2P_SYM(5) B2P_SYM(6)
+#undef B2P_BLOCK
+#undef B2P_SYM
+#undef B2P_ZARGS
+  set_error(op->ctx, "nd_hex_apply7z: no kernel for p=%d q1d=%d kind=%d", op->p, op->q1d, kind);
   return B2P_ERR_UNSUPPORTED;
 }
 

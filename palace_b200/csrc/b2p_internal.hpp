@@ -218,6 +218,11 @@ bool nd_tables_symmetric(const double *tab, int p, int q, double rel_tol);
 int launch_nd_hex_apply7(b2p_op *op, const int32_t *lidx, double alpha, const double *x, double *y, const ApplyRange &rg, cudaStream_t s,
                          bool transpose = false);
 bool nd_hex_apply7_eligible(b2p_op *op);
+// complex apply on nd_hex_apply7_kernel (p = 2 ... 6 for B2P_ND_BLOCK, 4 ... 6 for the symmetric kinds): coef is the 36-double
+// {mass Re, mass Im, curl Re, curl Im} block per element, or the real four-tensor block with coef_i the imaginary one;
+// y_r + i y_i += alpha (D_r + sgn i D_i) (x_r + i x_i) per element
+int launch_nd_hex_apply7z(b2p_op *op, int kind, const int32_t *lidx, const double *coef, const double *coef_i, int has_imag, double sgn,
+                          double alpha, const double *xr, const double *xi, double *yr, double *yi, cudaStream_t s);
 // fused complex apply (b2p_hex_nd4.cu): both parts of a split complex vector in one pass over the geometry
 bool nd_hex_apply4z_eligible(const b2p_op *op);
 int launch_nd_hex_apply4z(b2p_op *op, int kind, const int32_t *lidx, const double *zcoef, int has_imag, double alpha, const double *xr,
