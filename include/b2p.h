@@ -51,7 +51,14 @@ enum
    * hexahedra they also fuse with curl-curl / mass terms in b2p_op_create_sum. One coefficient context each, built by the
    * caller as the reference's integrators do (PopulateCoefficientContext with a = -1 for the weak curl, transpose for the curl): */
   B2P_ND_WEAKCURL = 4,   /* MixedVectorWeakCurlIntegrator: values -> curls,  f_apply_hcurlhdiv_33 (integ/mixedveccurl.cpp:68-117) */
-  B2P_ND_MIXEDCURL = 5   /* MixedVectorCurlIntegrator:     curls  -> values, f_apply_hdivhcurl_33 (integ/mixedveccurl.cpp:23-66)  */
+  B2P_ND_MIXEDCURL = 5,  /* MixedVectorCurlIntegrator:     curls  -> values, f_apply_hdivhcurl_33 (integ/mixedveccurl.cpp:23-66)  */
+  /* VectorFEMassIntegrator on a Raviart-Thomas (H(div)) space of hexahedra -> f_apply_hdiv_33 (integ/vecfemass.cpp:80-86):
+   * D = (w / detJ) J^T C J with the ND_MASS coefficient context. b2p_op_desc.p is the ND-equivalent order: the space is RT_{p-1},
+   * P = 3 p^2 (p + 1) dofs per element, restriction in the lexicographic RT layout (component c closed along axis c, open along the
+   * other two), Bo / Bc as for ND, Gc not read. Sum-factorised only (b2p_op_create, b2p_op_coarsen; b2p_op_create_dense refuses
+   * it); on-the-fly coefficients only (assemble_qdata = 1 returns B2P_ERR_UNSUPPORTED); single partition (b2p_op_apply_add_split
+   * with ghost pieces returns B2P_ERR_UNSUPPORTED); not a term of b2p_op_create_sum or b2p_coperator_par (B2P_ERR_UNSUPPORTED). */
+  B2P_RT_MASS = 6
 };
 
 /* ---- context -------------------------------------------------------------------------------- */
@@ -593,6 +600,14 @@ int b2p_flux_estimator_indicator(b2p_flux_estimator *e, const double *flux_re, c
 /* estimates[i] = sqrt(s estimates[i]): last step when several flux terms are added before the square root
  * (TimeDependentFluxErrorEstimator: project + integrate of both estimators into one array, errorestimator.cpp:531-545) */
 int b2p_flux_estimator_sqrt_scale(b2p_ctx *ctx, int64_t n, double s, double *estimates);
+/* FluxProjector with "EstimatorMG" (ConfigureLinearSolver(use_mg = true), errorestimator.cpp:66-100): the projection's PCG is
+ * preconditioned by GeometricMultigridSolver(coarse, P, no auxiliary space, 1 cycle, 1 smoothing iteration, 4th-kind Chebyshev of
+ * order 2, sf_max 1, sf_min 0) over the smooth space's p-hierarchy -- RT levels for the grad-flux estimator, ND levels for the
+ * curl-flux estimator; with one level the coarse solver alone. ops[n_levels] coarse -> fine (ops[n_levels-1] must be the
+ * estimator's smooth_mass), P[n_levels-1] the prolongations; coarse_type / coarse_tol / coarse_max_it / coarse_solver as in
+ * b2p_ksp_config and b2p_ksp_create. Replaces the Jacobi-preconditioned PCG; tolerances and the statistics stay. */
+int b2p_flux_estimator_set_multigrid(b2p_flux_estimator *e, int n_levels, b2p_operator *const *ops, b2p_operator *const *P, int coarse_type,
+                                     double coarse_tol, int coarse_max_it, b2p_solver *coarse_solver);
 int b2p_flux_estimator_stats(b2p_flux_estimator *e, int *num_mult, int *num_mult_its, int *last_its, int *converged);
 void b2p_flux_estimator_destroy(b2p_flux_estimator *e);
 

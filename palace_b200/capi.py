@@ -16,6 +16,8 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libb2p.so")
 
 CURLCURL, ND_MASS, CURLCURL_MASS, H1_DIFFUSION, ND_WEAKCURL, ND_MIXEDCURL = 0, 1, 2, 3, 4, 5
+# Raviart-Thomas mass on hexahedra: p is the ND-equivalent order (RT_{p-1}), Gc is not read (may be None)
+RT_MASS = 6
 
 _lib = None
 
@@ -1058,6 +1060,17 @@ class FluxEstimator:
     def indicator(self, flux_re, flux_im, Et, estimates):
         _chk(lib().b2p_flux_estimator_indicator(self.h, _vp(flux_re), _vp(flux_im) if flux_im is not None else None, C.c_double(Et),
                                                 _vp(estimates)), self.ctx.h)
+
+    def set_multigrid(self, ops, P, coarse_type=1, coarse_tol=1e-3, coarse_max_it=500, coarse_solver=None):
+        """FluxProjector with "EstimatorMG": PCG preconditioned by the p-multigrid over ops (Operators, coarse -> fine, the last one
+        the smooth-space mass operator given at construction) with the prolongations P (len(ops) - 1 Operators)."""
+        n = len(ops)
+        assert len(P) == n - 1
+        A = (C.c_void_p * n)(*[a.h for a in ops])
+        Parr = (C.c_void_p * max(1, len(P)))(*[p.h for p in P])
+        _chk(lib().b2p_flux_estimator_set_multigrid(self.h, n, A, Parr, int(coarse_type), C.c_double(coarse_tol), int(coarse_max_it),
+                                                    coarse_solver.h if coarse_solver else None), self.ctx.h)
+        self._keep.append([list(ops), list(P), coarse_solver])
 
     def stats(self):
         nm, nit, its, conv = C.c_int(), C.c_int(), C.c_int(), C.c_int()

@@ -449,6 +449,11 @@ struct b2p_ksp
   int ksp_mult = 0, ksp_mult_it = 0;
 };
 
+namespace b2p
+{
+IterativeSolver *ksp_solver_of(b2p_ksp *k) { return k ? k->ksp.get() : nullptr; }  // (the flux estimator's multigrid PCG)
+}
+
 extern "C"
 {
 

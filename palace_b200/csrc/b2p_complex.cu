@@ -1638,6 +1638,8 @@ int b2p_coperator_par(b2p_ctx *ctx, int64_t tsize, int64_t lsize, int n_terms, b
   for (int i = 0; i < n_terms; i++)
   {
     B2P_CHECK(ctx, ops[i] && b2p_op_lsize(ops[i]) == lsize, B2P_ERR_ARG, "b2p_coperator_par: term %d has the wrong L-size", i);
+    B2P_CHECK(ctx, ops[i]->kind != B2P_RT_MASS, B2P_ERR_UNSUPPORTED,
+              "b2p_coperator_par: term %d is a Raviart-Thomas operator; complex sums of them are not supported", i);
     B2P_CHECK(ctx, !ops[i]->lidx_bc || op_essential_matches(ops[i], ess_tdofs, n_ess), B2P_ERR_ARG,
               "b2p_coperator_par: term %d already carries a different essential-dof mask (one b2p_op = one essential set)", i);
     terms.push_back({ops[i], coef_re[i], coef_im[i]});

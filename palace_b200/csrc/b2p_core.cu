@@ -99,6 +99,13 @@ int apply_range(b2p_op *op, const int32_t *lidx, double alpha, const double *x, 
                 cudaStream_t s)
 {
   if (op->dense) return launch_dense_apply(op, lidx, alpha, x, y, rg, s, (flags & B2P_APPLY_TRANSPOSE) != 0);
+  // Raviart-Thomas mass (symmetric: the transpose flag changes nothing): rt_hex_apply7_kernel at p = 2 ... 6, q1d = p + 1 with
+  // mirror-symmetric tables, the cross-check kernel for everything else and under B2P_APPLY_SIMPLE_KERNEL. Single partition only.
+  if (op->kind == B2P_RT_MASS)
+  {
+    B2P_CHECK(op->ctx, !rg.xg && !rg.yg, B2P_ERR_UNSUPPORTED, "Raviart-Thomas operators: partitioned applies (ghost pieces) are not supported");
+    return launch_rt_hex_apply(op, lidx, alpha, x, y, rg, s, (flags & B2P_APPLY_SIMPLE_KERNEL) != 0);
+  }
   // Block operators (mixed curl kinds on hexes and sums containing one): nd_hex_apply6_kernel (p = 2, 3) or
   // nd_hex_apply7_kernel (p = 4, 5, 6) at q1d = p + 1 with mirror-symmetric tables, the cross-check kernel for everything else
   // and whenever an apply flag asks for another kernel (there is no block form in nd_hex_apply4/5_kernel).
@@ -488,7 +495,12 @@ int set_coeff(b2p_op *op, const void *blob, size_t bytes)
   return B2P_SUCCESS;
 }
 
-int elem_dofs(int kind, int p) { return kind == B2P_H1_DIFFUSION ? (p + 1) * (p + 1) * (p + 1) : 3 * p * (p + 1) * (p + 1); }
+int elem_dofs(int kind, int p)
+{
+  if (kind == B2P_H1_DIFFUSION) return (p + 1) * (p + 1) * (p + 1);
+  if (kind == B2P_RT_MASS) return 3 * p * p * (p + 1);  // RT_{p-1}: closed along one axis, open along two
+  return 3 * p * (p + 1) * (p + 1);
+}
 
 // Compose the native-order restriction + orientation with the lexicographic->native dof map
 // (restriction.cpp:134-188,281-297) into one signed lexicographic index array.
@@ -529,9 +541,10 @@ int build_tables(b2p_op *op, const b2p_op_desc *d)
     B2P_CHECK(op->ctx, d->Bo, B2P_ERR_ARG, "Bo table required for ND operators");
     std::memcpy(tab.data(), d->Bo, sizeof(double) * q * p);
   }
-  B2P_CHECK(op->ctx, d->Bc && d->Gc, B2P_ERR_ARG, "Bc/Gc tables required");
+  const bool need_g = op->kind != B2P_RT_MASS;  // the RT mass reads values only
+  B2P_CHECK(op->ctx, d->Bc && (d->Gc || !need_g), B2P_ERR_ARG, "Bc/Gc tables required");
   std::memcpy(tab.data() + (size_t)q * p, d->Bc, sizeof(double) * q * n);
-  std::memcpy(tab.data() + (size_t)q * p + (size_t)q * n, d->Gc, sizeof(double) * q * n);
+  if (need_g) std::memcpy(tab.data() + (size_t)q * p + (size_t)q * n, d->Gc, sizeof(double) * q * n);
   op->h_tab = tab;
   return upload(op->ctx, tab.data(), tab.size(), &op->tab);
 }
@@ -557,9 +570,11 @@ int assemble_qdata(b2p_op *op)
 int b2p_op_create(b2p_ctx *ctx, b2p_geom *geom, const b2p_op_desc *d, b2p_op **out)
 {
   B2P_CHECK(ctx, ctx && geom && d && out, B2P_ERR_ARG, "b2p_op_create: null argument");
-  B2P_CHECK(ctx, d->kind >= B2P_CURLCURL && d->kind <= B2P_ND_MIXEDCURL, B2P_ERR_ARG, "b2p_op_create: bad kind %d", d->kind);
+  B2P_CHECK(ctx, d->kind >= B2P_CURLCURL && d->kind <= B2P_RT_MASS, B2P_ERR_ARG, "b2p_op_create: bad kind %d", d->kind);
   B2P_CHECK(ctx, !(d->assemble_qdata && (d->kind == B2P_ND_WEAKCURL || d->kind == B2P_ND_MIXEDCURL)), B2P_ERR_UNSUPPORTED,
             "b2p_op_create: assembled q-data is not available for the mixed curl kinds (apply their coefficient on the fly)");
+  B2P_CHECK(ctx, !(d->assemble_qdata && d->kind == B2P_RT_MASS), B2P_ERR_UNSUPPORTED,
+            "b2p_op_create: assembled q-data is not available for the Raviart-Thomas mass (apply its coefficient on the fly)");
   B2P_CHECK(ctx, d->ne == geom->ne, B2P_ERR_ARG, "b2p_op_create: %d elements vs %d in geometry", d->ne, geom->ne);
   B2P_CHECK(ctx, d->p >= 1 && d->p <= 6 && d->p < geom->q1d && geom->q1d <= 7, B2P_ERR_UNSUPPORTED,
             "b2p_op_create: unsupported p=%d q1d=%d (hex kernels cover p<=6, p<q1d<=7)", d->p, geom->q1d);
@@ -754,7 +769,7 @@ int b2p_op_apply_add_pair(b2p_op *op, double alpha, const double *x0, const doub
     B2P_CHECK(op->ctx, op->lidx_bc, B2P_ERR_ARG, "b2p_op_apply_add_pair: masked apply without b2p_op_set_essential");
     lidx = op->lidx_bc;
   }
-  if (op->bcoef || !nd_hex_apply4z_eligible(op) || !op->ecoef)
+  if (op->bcoef || op->kind == B2P_RT_MASS || !nd_hex_apply4z_eligible(op) || !op->ecoef)
   {
     int rc = b2p::apply_range(op, lidx, alpha, x0, y0, ApplyRange(), flags, (cudaStream_t)s);
     return rc ? rc : b2p::apply_range(op, lidx, alpha, x1, y1, ApplyRange(), flags, (cudaStream_t)s);
@@ -845,6 +860,7 @@ int b2p_op_diag_add(b2p_op *op, double *diag, b2p_stream s)
   if (!op || !diag) return B2P_ERR_ARG;
   if (op->dense) return launch_dense_diag(op, diag, (cudaStream_t)s);
   if (op->kind == B2P_H1_DIFFUSION) return launch_h1_hex_diag(op, diag, (cudaStream_t)s);
+  if (op->kind == B2P_RT_MASS) return launch_rt_hex_diag(op, diag, (cudaStream_t)s);
   return launch_nd_hex_diag(op, diag, (cudaStream_t)s);
 }
 

@@ -29,6 +29,7 @@ namespace b2p
 {
 Operator *operator_of(b2p_operator *A);
 b2p_operator *wrap_operator(std::unique_ptr<Operator> &&op);
+IterativeSolver *ksp_solver_of(b2p_ksp *k);
 }
 
 namespace b2p
@@ -367,10 +368,13 @@ struct b2p_flux_estimator
   const Operator *M = nullptr;
   std::unique_ptr<JacobiSmoother> pc;
   std::unique_ptr<IterativeSolver> pcg;
+  b2p_ksp *mg = nullptr;                 // b2p_flux_estimator_set_multigrid: PCG with the geometric multigrid preconditioner
+  IterativeSolver *solver = nullptr;     // the projection's solver: pcg, or the one inside mg
   DVec rhs, H;
   int mult = 0, mult_it = 0;
   ~b2p_flux_estimator()
   {
+    b2p_ksp_destroy(mg);
     cudaFree(flux.interp);
     cudaFree(flux.sidx);
     cudaFree(flux.co);
@@ -448,6 +452,7 @@ int b2p_flux_estimator_create(b2p_ctx *ctx, b2p_geom *geom, const b2p_vecfe_spac
   e->pcg->max_it = max_it;
   e->pcg->SetOperator(*M);
   e->pcg->SetPreconditioner(e->pc.get());
+  e->solver = e->pcg.get();
   cudaError_t err = cudaPeekAtLastError();
   B2P_CHECK(ctx, err == cudaSuccess, B2P_ERR_CUDA, "b2p_flux_estimator_create: %s", cudaGetErrorString(err));
   *out = e.release();
@@ -461,12 +466,12 @@ int b2p_flux_estimator_project(b2p_flux_estimator *e, const double *flux_dofs, d
   b2p_ctx *ctx = e->ctx;
   if (e->rhs.n != e->smooth.lsize) e->rhs.resize(ctx, e->smooth.lsize);
   e->Flux->Mult(flux_dofs, e->rhs.p);
-  e->pcg->Mult(e->rhs.p, smooth_dofs);
-  if (!e->pcg->converged)
-    set_error(ctx, "Linear solver did not converge, norm(Ax-b)/norm(b) = %.3e (norm(b) = %.3e)!", e->pcg->final_res / e->pcg->initial_res,
-              e->pcg->initial_res);
+  e->solver->Mult(e->rhs.p, smooth_dofs);
+  if (!e->solver->converged)
+    set_error(ctx, "Linear solver did not converge, norm(Ax-b)/norm(b) = %.3e (norm(b) = %.3e)!", e->solver->final_res / e->solver->initial_res,
+              e->solver->initial_res);
   e->mult++;
-  e->mult_it += e->pcg->final_it;
+  e->mult_it += e->solver->final_it;
   cudaError_t err = cudaPeekAtLastError();
   B2P_CHECK(ctx, err == cudaSuccess, B2P_ERR_CUDA, "b2p_flux_estimator_project: %s", cudaGetErrorString(err));
   return B2P_SUCCESS;
@@ -510,8 +515,50 @@ int b2p_flux_estimator_stats(b2p_flux_estimator *e, int *num_mult, int *num_mult
   if (!e) return B2P_ERR_ARG;
   if (num_mult) *num_mult = e->mult;
   if (num_mult_its) *num_mult_its = e->mult_it;
-  if (last_its) *last_its = e->pcg->final_it;
-  if (converged) *converged = e->pcg->converged ? 1 : 0;
+  if (last_its) *last_its = e->solver->final_it;
+  if (converged) *converged = e->solver->converged ? 1 : 0;
+  return B2P_SUCCESS;
+}
+
+// ConfigureLinearSolver(use_mg = true) (errorestimator.cpp:66-100): PCG, no initial guess, the estimator's relative tolerance,
+// absolute tolerance epsilon; preconditioner GeometricMultigridSolver(coarse, P, no auxiliary space, 1 cycle, 1 smoothing
+// iteration, 4th-kind Chebyshev of order 2, sf_max 1, sf_min 0), or the coarse solver alone on one level.
+int b2p_flux_estimator_set_multigrid(b2p_flux_estimator *e, int n_levels, b2p_operator *const *ops, b2p_operator *const *P, int coarse_type,
+                                     double coarse_tol, int coarse_max_it, b2p_solver *coarse_solver)
+{
+  if (!e) return B2P_ERR_ARG;
+  b2p_ctx *ctx = e->ctx;
+  B2P_CHECK(ctx, n_levels >= 1 && ops && (n_levels == 1 || P), B2P_ERR_ARG, "b2p_flux_estimator_set_multigrid: bad argument");
+  B2P_CHECK(ctx, ops[n_levels - 1] && operator_of(ops[n_levels - 1]) == e->M, B2P_ERR_ARG,
+            "b2p_flux_estimator_set_multigrid: the finest level operator must be the estimator's smooth-space mass operator");
+  b2p_ksp_config cfg;
+  b2p_ksp_config_default(&cfg, 1);
+  cfg.krylov_solver = 0;
+  cfg.tol = e->pcg->rel_tol;
+  cfg.max_it = e->pcg->max_it;
+  cfg.initial_guess = 0;
+  cfg.mg_cycle_it = 1;
+  cfg.mg_smooth_aux = 0;
+  cfg.mg_smooth_it = 1;
+  cfg.mg_smooth_order = 2;
+  cfg.mg_smooth_sf_max = 1.0;
+  cfg.mg_smooth_sf_min = 0.0;
+  cfg.mg_smooth_cheby_4th = 1;
+  cfg.coarse_type = coarse_type;
+  cfg.coarse_tol = coarse_tol;
+  cfg.coarse_max_it = coarse_max_it;
+  b2p_ksp *k = nullptr;
+  int rc = b2p_ksp_create(ctx, &cfg, n_levels, P, nullptr, coarse_solver, &k);
+  if (rc) return rc;
+  ksp_solver_of(k)->abs_tol = e->pcg->abs_tol;
+  if ((rc = b2p_ksp_set_operators(k, ops[n_levels - 1], ops, nullptr)))
+  {
+    b2p_ksp_destroy(k);
+    return rc;
+  }
+  b2p_ksp_destroy(e->mg);
+  e->mg = k;
+  e->solver = ksp_solver_of(k);
   return B2P_SUCCESS;
 }
 

@@ -232,6 +232,12 @@ bool op_essential_matches(const b2p_op *op, const int32_t *ess_ldofs, int64_t n)
 int apply_range(b2p_op *op, const int32_t *lidx, double alpha, const double *x, double *y, const ApplyRange &rg, int flags,
                 cudaStream_t s);
 int launch_nd_hex_diag(b2p_op *op, double *diag, cudaStream_t s);
+// Raviart-Thomas mass (b2p_hex_rt.cu): the production kernel where rt_hex_apply7_eligible holds and `simple` is not set, the
+// cross-check kernel otherwise
+bool rt_hex_apply7_eligible(b2p_op *op);
+int launch_rt_hex_apply(b2p_op *op, const int32_t *lidx, double alpha, const double *x, double *y, const ApplyRange &rg, cudaStream_t s,
+                        bool simple);
+int launch_rt_hex_diag(b2p_op *op, double *diag, cudaStream_t s);
 int launch_h1_hex_apply(b2p_op *op, const int32_t *lidx, double alpha, const double *x, double *y, const ApplyRange &rg, cudaStream_t s);
 int launch_h1_hex_apply3(b2p_op *op, const int32_t *lidx, double alpha, const double *x, double *y, const ApplyRange &rg,
                          cudaStream_t s);

@@ -22,6 +22,8 @@ def space_dict(sp: hs.HexSpace):
     if sp.kind == "nd":
         idx, ori = sp.native_restriction()
         return dict(P=sp.P, lsize=sp.ndofs, idx=idx, orient=ori, dof_map=sp.dof_map)
+    if sp.kind == "rt":  # lexicographic is native here; the face dofs carry their orientation sign
+        return dict(P=sp.P, lsize=sp.ndofs, idx=sp.lex_gid.astype(np.int32), orient=sp.lex_sign, dof_map=None)
     return dict(P=sp.P, lsize=sp.ndofs, idx=sp.lex_gid.astype(np.int32), orient=None, dof_map=None)
 
 
@@ -43,6 +45,27 @@ def nd_prolongation_comps(pc, pf):
         in_n[c], out_n[c] = pc, pf
         A = [Cc, Cc, Cc]
         A[c] = Oo
+        comps.append(dict(in_off=c * d3c, in_n=in_n, out_off=c * d3f, out_n=out_n, A=A))
+    return comps
+
+
+def rt_prolongation_comps(pc, pf):
+    """Kronecker factors of the RT hex p-prolongation (hexspace.rt_prolongation_matrix): per vector component, closed-basis
+    interpolation along its own axis and open-basis along the other two."""
+    opc, _ = hs.gauss_legendre(pc)
+    cpc = hs.gauss_lobatto(pc + 1)
+    opf, _ = hs.gauss_legendre(pf)
+    cpf = hs.gauss_lobatto(pf + 1)
+    Oo, _ = hs.lagrange_table(opc, opf)  # [pf, pc]
+    Cc, _ = hs.lagrange_table(cpc, cpf)  # [pf+1, pc+1]
+    d3c, d3f = (pc + 1) * pc * pc, (pf + 1) * pf * pf
+    comps = []
+    for c in range(3):
+        in_n = [pc] * 3
+        out_n = [pf] * 3
+        in_n[c], out_n[c] = pc + 1, pf + 1
+        A = [Oo, Oo, Oo]
+        A[c] = Cc
         comps.append(dict(in_off=c * d3c, in_n=in_n, out_off=c * d3f, out_n=out_n, A=A))
     return comps
 

@@ -537,6 +537,30 @@ def build_rt_space(mesh: HexMesh, topo: HexTopology, p: int) -> HexSpace:
     return HexSpace("rt", p, ndofs, P, gid, sgn, np.arange(P, dtype=np.int64), np.nonzero(ess)[0], mult)
 
 
+def rt_prolongation_matrix(pc: int, pf: int) -> np.ndarray:
+    """I[l_f, m_c] = fine RT dof functional l_f applied to coarse RT shape function m_c (GetTransferMatrix semantics), lexicographic on
+    both sides: per component, closed (Gauss-Lobatto) interpolation along its own axis and open (Gauss-Legendre) along the other two
+    -- ND's assignment (nd_prolongation_matrix) with the roles exchanged."""
+    opc, _ = gauss_legendre(pc)
+    cpc = gauss_lobatto(pc + 1)
+    opf, _ = gauss_legendre(pf)
+    cpf = gauss_lobatto(pf + 1)
+    Oo, _ = lagrange_table(opc, opf)  # [pf, pc]
+    Cc, _ = lagrange_table(cpc, cpf)  # [pf+1, pc+1]
+    lay_f = _rt_lex_layout(pf)
+    lay_c = _rt_lex_layout(pc)
+    I = np.zeros((len(lay_f), len(lay_c)))
+    for lf, (c, i, j, k) in enumerate(lay_f):
+        for mc, (c2, i2, j2, k2) in enumerate(lay_c):
+            if c != c2:
+                continue
+            tx = Cc[i, i2] if c == 0 else Oo[i, i2]
+            ty = Cc[j, j2] if c == 1 else Oo[j, j2]
+            tz = Cc[k, k2] if c == 2 else Oo[k, k2]
+            I[lf, mc] = tx * ty * tz
+    return I
+
+
 def rt_hex_dense_interp(p: int, q1d: int) -> np.ndarray:
     """interp[3][Q][P]: reference-space values of the lexicographic RT basis at the tensor Gauss-Legendre points (x fastest),
     the layout of libCEED non-tensor bases (fem/libceed/basis.cpp:40-85)."""
