@@ -73,6 +73,23 @@ int b2p_ctx_rank(b2p_ctx *ctx);
 int b2p_ctx_nranks(b2p_ctx *ctx);
 int b2p_ctx_sync(b2p_ctx *ctx, b2p_stream s);
 
+/* Launch record of the persistent element kernels (nd_hex_apply4/5/6/7_kernel, h1_hex_apply3_kernel). Each of them clamps its
+ * grid to the element batches and lets every worker (a warp, or the whole CTA for nd_hex_apply7_kernel) walk batch, batch + W,
+ * ... with W workers in the grid. The launcher stores, on the host, what it launched last on this context, whichever operator
+ * or complex / true-dof wrapper asked for it: which kernel ran, and whether every worker saw several batches. */
+typedef struct
+{
+  char kernel[48];      /* kernel name and form: "nd_hex_apply7_kernel", "nd_hex_apply7_kernel:block", "...:cplx", "...:block:cplx" */
+  int max_grid;         /* SM count x CTAs per SM: the grid before clamping to the batches */
+  int grid;             /* CTAs launched */
+  int workers;          /* batch walkers per CTA: warps (nd4, nd5, nd6, h1v3) or 1 (nd7) */
+  int elems_per_batch;  /* elements of one batch */
+  int64_t batches;      /* batches of the launch (the last one may be partly filled) */
+  int64_t seq;          /* persistent launches recorded on this context so far, this one included */
+} b2p_launch_info;
+/* B2P_ERR_ARG before the first persistent launch on ctx. */
+int b2p_ctx_last_launch(b2p_ctx *ctx, b2p_launch_info *out);
+
 /* ---- device memory helpers (so a C/C++ host needs no CUDA runtime of its own) ----------------- */
 int b2p_malloc(b2p_ctx *ctx, size_t bytes, void **dptr);
 int b2p_free(b2p_ctx *ctx, void *dptr);

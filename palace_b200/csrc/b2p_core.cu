@@ -222,6 +222,14 @@ const char *b2p_last_error(b2p_ctx *ctx) { return ctx ? ctx->last_error.c_str() 
 int b2p_ctx_rank(b2p_ctx *ctx) { return ctx ? ctx->rank : 0; }
 int b2p_ctx_nranks(b2p_ctx *ctx) { return ctx ? ctx->nranks : 1; }
 
+int b2p_ctx_last_launch(b2p_ctx *ctx, b2p_launch_info *out)
+{
+  if (!ctx || !out) return B2P_ERR_ARG;
+  B2P_CHECK(ctx, ctx->last_launch.seq > 0, B2P_ERR_ARG, "b2p_ctx_last_launch: no persistent element kernel launched on this context yet");
+  *out = ctx->last_launch;
+  return B2P_SUCCESS;
+}
+
 int b2p_ctx_sync(b2p_ctx *ctx, b2p_stream s)
 {
   B2P_CUDA(ctx, cudaStreamSynchronize((cudaStream_t)s));

@@ -437,6 +437,7 @@ int launch_h1v3(b2p_op *op, const int32_t *lidx, double alpha, const double *x, 
   const int nb = (e_cnt + L::NEW - 1) / L::NEW;
   int grid = op->ctx->sm_count * MINB;
   if (grid > (nb + NW - 1) / NW) grid = (nb + NW - 1) / NW;
+  record_launch(op->ctx, "h1_hex_apply3_kernel", false, false, op->ctx->sm_count * MINB, grid, NW, L::NEW, nb);
   B2P_LAUNCH(kern, grid, NW * 32, shmem, s, prm);
   B2P_CUDA(op->ctx, cudaGetLastError());
   return B2P_SUCCESS;

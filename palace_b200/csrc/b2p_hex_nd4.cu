@@ -935,6 +935,7 @@ int launch4(b2p_op *op, const int32_t *lidx, double alpha, const double *x, doub
   const int nb = (e_cnt + L::NEW - 1) / L::NEW;
   int grid = op->ctx->sm_count * MINB;
   if (grid > (nb + NW - 1) / NW) grid = (nb + NW - 1) / NW;
+  record_launch(op->ctx, "nd_hex_apply4_kernel", false, false, op->ctx->sm_count * MINB, grid, NW, L::NEW, nb);
   if (rg.pdl)
     B2P_LAUNCH_PDL(kern, grid, NW * 32, shmem, s, prm);
   else
@@ -1020,6 +1021,7 @@ int launch4z(b2p_op *op, const int32_t *lidx, const double *zcoef, int has_imag,
     const int nb = (op->ne + L::NEB - 1) / L::NEB;
     int grid = op->ctx->sm_count * MINB;
     if (grid > (nb + NW - 1) / NW) grid = (nb + NW - 1) / NW;
+    record_launch(op->ctx, "nd_hex_apply4_kernel", false, true, op->ctx->sm_count * MINB, grid, NW, L::NEB, nb);
     B2P_LAUNCH(kern, grid, NW * 32, shmem, s, prm);
     B2P_CUDA(op->ctx, cudaGetLastError());
     return B2P_SUCCESS;

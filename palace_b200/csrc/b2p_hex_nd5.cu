@@ -691,6 +691,7 @@ int launch5(b2p_op *op, const int32_t *lidx, double alpha, const double *x, doub
   for (int i = 0; i < q * n; i++) prm.Gc[i] = op->h_tab[q * P_ + q * n + i];
   int grid = op->ctx->sm_count * MINB;
   if (grid > (e_cnt + NW - 1) / NW) grid = (e_cnt + NW - 1) / NW;
+  record_launch(op->ctx, "nd_hex_apply5_kernel", false, false, op->ctx->sm_count * MINB, grid, NW, 1, e_cnt);
   B2P_LAUNCH(kern, grid, NW * 32, shmem, s, prm);
   B2P_CUDA(op->ctx, cudaGetLastError());
   return B2P_SUCCESS;

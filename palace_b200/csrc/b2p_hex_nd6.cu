@@ -957,6 +957,7 @@ int launch6_cfg(b2p_op *op, const int32_t *lidx, double alpha, const double *x, 
   const int nb = (e_cnt + L::NEW - 1) / L::NEW;
   int grid = op->ctx->sm_count * MINB;
   if (grid > (nb + NW - 1) / NW) grid = (nb + NW - 1) / NW;
+  record_launch(op->ctx, "nd_hex_apply6_kernel", L::BLOCK, false, op->ctx->sm_count * MINB, grid, NW, L::NEW, nb);
   if (rg.pdl)
     B2P_LAUNCH_PDL(kern, grid, NW * 32, shmem, s, prm);
   else

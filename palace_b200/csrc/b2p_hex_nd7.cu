@@ -966,6 +966,7 @@ int launch7_cfg(b2p_op *op, const int32_t *lidx, double alpha, const double *x, 
   const int nb = (e_cnt + NE - 1) / NE;
   int grid = op->ctx->sm_count * MINB;
   if (grid > nb) grid = nb;
+  record_launch(op->ctx, "nd_hex_apply7_kernel", L::BLOCK, false, op->ctx->sm_count * MINB, grid, 1, NE, nb);
   if (rg.pdl)
     B2P_LAUNCH_PDL(kern, grid, NT, shmem, s, prm);
   else
@@ -1020,6 +1021,7 @@ int launch7z(b2p_op *op, const int32_t *lidx, const double *coef, const double *
   const int nb = (op->ne + S::NE - 1) / S::NE;
   int grid = op->ctx->sm_count * S::MINB_CPLX;
   if (grid > nb) grid = nb;
+  record_launch(op->ctx, "nd_hex_apply7_kernel", L::BLOCK, true, op->ctx->sm_count * S::MINB_CPLX, grid, 1, S::NE, nb);
   B2P_LAUNCH(kern, grid, NT, shmem, s, prm);
   B2P_CUDA(op->ctx, cudaGetLastError());
   return B2P_SUCCESS;

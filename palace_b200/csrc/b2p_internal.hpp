@@ -91,6 +91,8 @@ struct b2p_ctx
   // sink of the branch-free scatter (nd_hex_apply6_kernel): masked restriction entries add 0.0 to a per-thread slot here
   double *d_sink = nullptr;
   static constexpr int SINK_SLOTS = 1 << 16;
+  // what the last persistent element kernel launched on this context was (b2p_ctx_last_launch; host-side stores only)
+  b2p_launch_info last_launch = {};
 };
 
 // Geometry q-data of one element block, device resident.
@@ -204,6 +206,19 @@ constexpr int B2P_ND_BLOCK = 16;
 inline bool op_nonsymmetric(const b2p_op *op)
 {
   return op->kind == B2P_ND_WEAKCURL || op->kind == B2P_ND_MIXEDCURL || op->bcoef != nullptr;
+}
+// Store the launch record of a persistent element kernel on its context (b2p_ctx_last_launch). `block` / `cplx` name the form.
+inline void record_launch(b2p_ctx *c, const char *kernel, bool block, bool cplx, int max_grid, int grid, int workers, int elems_per_batch,
+                          int64_t batches)
+{
+  b2p_launch_info &r = c->last_launch;
+  snprintf(r.kernel, sizeof(r.kernel), "%s%s%s", kernel, block ? ":block" : "", cplx ? ":cplx" : "");
+  r.max_grid = max_grid;
+  r.grid = grid;
+  r.workers = workers;
+  r.elems_per_batch = elems_per_batch;
+  r.batches = batches;
+  r.seq++;
 }
 // Kernel launchers (defined in the .cu files).
 int launch_nd_hex_apply(b2p_op *op, const int32_t *lidx, double alpha, const double *x, double *y, const ApplyRange &rg, cudaStream_t s,

@@ -209,9 +209,13 @@ def test_h1_production_and_simple_kernels_agree_with_alpha_and_mask(b2p_ctx, p):
 @pytest.mark.parametrize("p", [2, 3])
 @pytest.mark.parametrize("kind", [O.CURLCURL, O.ND_MASS, O.CURLCURL_MASS])
 def test_both_production_nd_kernels_match_the_oracle(b2p_ctx, kind, p):
-    """p = 2, 3 run nd_hex_apply6_kernel by default (register x-gather, XDX on the Z region, aliased work arrays, half tables,
-    branch-free scatter); B2P_APPLY_ROUND1_KERNEL selects nd_hex_apply4_kernel for the same call. Both against the oracle: plain,
-    scaled + masked, and over element sub-ranges with the owned | ghost split (a ragged last batch in each piece)."""
+    """The default kernel -- nd_hex_apply7_kernel at p = 2 (one CTA per element batch, one 1-D line per thread), nd_hex_apply6_kernel
+    at p = 3 (register x-gather, XDX on the Z region, aliased work arrays, half tables, branch-free scatter) -- and
+    nd_hex_apply4_kernel, which B2P_APPLY_ROUND1_KERNEL selects for the same call. Both against the oracle: plain, scaled +
+    masked, and over element sub-ranges with the owned | ghost split (a ragged last batch in each piece). The launch record says
+    which kernel ran."""
+    from palace_b200 import capi
+
     prob = common.make_problem(n=(3, 3, 2), p=p)
     blob = common.coefficient(kind, 3, "matrix", a_mass=0.9, a_curl=1.1)
     g = common.gpu_geom(b2p_ctx, prob)
@@ -231,6 +235,7 @@ def test_both_production_nd_kernels_match_the_oracle(b2p_ctx, kind, p):
         yd = _dev(y0)
         op.apply_add_ex(1.5, _dev(x), yd, round1_kernel=r1)
         assert _rel(yd.cpu().numpy(), y0 + 1.5 * y_ref) < RTOL
+        assert capi.last_launch(b2p_ctx)["kernel"] == ("nd_hex_apply4_kernel" if r1 else {2: "nd_hex_apply7_kernel", 3: "nd_hex_apply6_kernel"}[p])
         yd = _dev(y0)
         op.apply_add_ex(-0.5, _dev(x), yd, masked=True, round1_kernel=r1)
         assert _rel(yd.cpu().numpy(), y0 - 0.5 * ym) < RTOL

@@ -13,8 +13,8 @@ import pytest
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
-def _run(files, order, extra=()):
-    env = dict(os.environ, B2P_EMU_TESTS="1", B2P_EMU_ORDER=order)
+def _run(files, order, extra=(), env=None):
+    env = dict(os.environ, B2P_EMU_TESTS="1", B2P_EMU_ORDER=order, **(env or {}))
     cmd = [sys.executable, "-m", "pytest", "-m", "gpu", "-q", "-x", "-p", "no:cacheprovider", *extra, *files]
     r = subprocess.run(cmd, cwd=ROOT, env=env, capture_output=True, text=True, timeout=1500)
     tail = (r.stdout + r.stderr)[-3000:]
@@ -40,6 +40,14 @@ def test_element_kernels_under_emulation(order):
     different lane execution orders (a missing warp barrier shows up as stale data in at least one of them)."""
     n = _run(["tests/test_apply_gpu.py", "tests/test_dense_gpu.py", "tests/test_tet_gpu.py", "tests/test_zfused_gpu.py", "tests/test_zassemble_gpu.py", "tests/test_zbdr_gpu.py", "tests/test_zsolver_variants_gpu.py", "tests/test_zsum_gpu.py"], order)
     assert n >= 120
+
+
+@pytest.mark.parametrize("order", ["fwd", "rev"])
+def test_persistent_kernels_in_steady_state_under_emulation(order):
+    """tests/test_zzsteady_state_gpu.py on ONE emulated SM: the meshes it sizes from the launch records stay small, and every
+    warp or CTA of the persistent ND / H1 hex kernels still walks several element batches (ring slots reused, mbarrier parities
+    flipped, next-batch prefetches), in both lane execution orders."""
+    assert _run(["tests/test_zzsteady_state_gpu.py"], order, env={"B2P_EMU_SMS": "1"}) >= 97
 
 
 def test_solver_layer_under_emulation():
