@@ -76,7 +76,9 @@ int b2p_ctx_sync(b2p_ctx *ctx, b2p_stream s);
 /* Launch record of the persistent element kernels (nd_hex_apply4/5/6/7_kernel, h1_hex_apply3_kernel). Each of them clamps its
  * grid to the element batches and lets every worker (a warp, or the whole CTA for nd_hex_apply7_kernel) walk batch, batch + W,
  * ... with W workers in the grid. The launcher stores, on the host, what it launched last on this context, whichever operator
- * or complex / true-dof wrapper asked for it: which kernel ran, and whether every worker saw several batches. */
+ * or complex / true-dof wrapper asked for it: which kernel ran, and whether every worker saw several batches. The kernels of
+ * the hexahedral flux estimator (flux_hex_mixed7 / error7 and their cross-check kernels flux_hex_mixed / error, one batch per
+ * CTA: grid = max_grid = batches, workers = 1) record themselves too, so a caller can see which route ran. */
 typedef struct
 {
   char kernel[48];      /* kernel name and form: "nd_hex_apply7_kernel", "nd_hex_apply7_kernel:block", "...:cplx", "...:block:cplx" */
@@ -85,7 +87,7 @@ typedef struct
   int workers;          /* batch walkers per CTA: warps (nd4, nd5, nd6, h1v3) or 1 (nd7) */
   int elems_per_batch;  /* elements of one batch */
   int64_t batches;      /* batches of the launch (the last one may be partly filled) */
-  int64_t seq;          /* persistent launches recorded on this context so far, this one included */
+  int64_t seq;          /* launches recorded on this context so far, this one included */
 } b2p_launch_info;
 /* B2P_ERR_ARG before the first persistent launch on ctx. */
 int b2p_ctx_last_launch(b2p_ctx *ctx, b2p_launch_info *out);
@@ -627,6 +629,21 @@ int b2p_flux_estimator_set_multigrid(b2p_flux_estimator *e, int n_levels, b2p_op
                                      double coarse_tol, int coarse_max_it, b2p_solver *coarse_solver);
 int b2p_flux_estimator_stats(b2p_flux_estimator *e, int *num_mult, int *num_mult_its, int *last_its, int *converged);
 void b2p_flux_estimator_destroy(b2p_flux_estimator *e);
+/* The flux estimator on hexahedra with sum-factorised spaces: flux_space / smooth_space are b2p_op_desc restricted to their
+ * space fields (kind = B2P_ND_MASS or B2P_RT_MASS names the space, one of each; p, ne, lsize, idx, orient, dof_map, Bo, Bc
+ * read as b2p_op_create reads them for that kind; coeff_ctx ignored; assemble_qdata must be 0). geom: tensor q-data (q1d > 0).
+ * Both spaces are evaluated with the same 1-D tables: the smooth space's Bo / Bc must equal the flux space's (B2P_ERR_ARG otherwise).
+ * Coefficient tables, smooth_mass, tol, max_it and the returned handle as b2p_flux_estimator_create. Flux and the error integrals
+ * run the sum-factorised kernels of b2p_hex_flux.cu (both directions, general coefficient matrices); project, integrate, indicator,
+ * set_multigrid, stats and destroy work on it unchanged. B2P_ERR_ARG: a kind other than ND_MASS / RT_MASS, two spaces of the same
+ * type, different p, ne different from the geometry's, a geometry without tensor q-data, smooth_mass of the wrong size, different
+ * tables, a restriction index outside [0, lsize); B2P_ERR_UNSUPPORTED: assemble_qdata = 1, nranks > 1, p / q1d outside the hex
+ * kernels. The kinds are checked first, so a wrong kind is B2P_ERR_ARG whatever else the description holds. */
+int b2p_flux_estimator_create_hex(b2p_ctx *ctx, b2p_geom *geom, const b2p_op_desc *flux_space, const b2p_op_desc *smooth_space,
+                                  int n_attr, const double *coef_flux, const double *coef_disc, const double *coef_smooth,
+                                  b2p_operator *smooth_mass, double tol, int max_it, b2p_flux_estimator **out);
+/* rhs = Flux flux_dofs (the projection's right-hand side), for estimators from either create function */
+int b2p_flux_estimator_flux_mult(b2p_flux_estimator *e, const double *flux_dofs, double *rhs);
 
 #ifdef __cplusplus
 }

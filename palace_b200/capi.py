@@ -1066,6 +1066,36 @@ class FluxEstimator:
                                              smooth_mass.h, C.c_double(tol), int(max_it), C.byref(self.h)), ctx.h)
         self._keep = [geom, smooth_mass, keep]
 
+    @classmethod
+    def hex(cls, ctx, geom, flux_space, smooth_space, coef_flux, coef_disc, coef_smooth, smooth_mass, tol=1e-6, max_it=500):
+        """b2p_flux_estimator_create_hex: the same estimator on hexahedra with sum-factorised spaces. flux_space / smooth_space are
+        dicts of the fields Op.create takes (kind = ND_MASS or RT_MASS, one of each; p, lsize, idx, orient, dof_map, Bo, Bc;
+        Gc, coeff and assemble optional)."""
+        self = cls.__new__(cls)
+        self.ctx = ctx
+        keep = []
+
+        def desc(sp):
+            d, k = _desc(sp["kind"], sp["p"], sp["lsize"], sp["idx"], sp.get("orient"), sp.get("dof_map"), sp.get("Bo"), sp.get("Bc"),
+                         sp.get("Gc"), sp.get("coeff"), sp.get("assemble", False))
+            keep.append(k)
+            return d
+
+        d1, d2 = desc(flux_space), desc(smooth_space)
+        cf = np.ascontiguousarray(coef_flux, dtype=np.float64).reshape(-1, 9)
+        cd = np.ascontiguousarray(coef_disc, dtype=np.float64).reshape(-1, 9)
+        cs = np.ascontiguousarray(coef_smooth, dtype=np.float64).reshape(-1, 9)
+        assert cf.shape == cd.shape == cs.shape
+        self.h = C.c_void_p()
+        _chk(lib().b2p_flux_estimator_create_hex(ctx.h, geom.h, C.byref(d1), C.byref(d2), int(cf.shape[0]), _ptr(cf), _ptr(cd), _ptr(cs),
+                                                 smooth_mass.h, C.c_double(tol), int(max_it), C.byref(self.h)), ctx.h)
+        self._keep = [geom, smooth_mass, keep]
+        return self
+
+    def flux_mult(self, flux_dofs, rhs):
+        """rhs = Flux flux_dofs: the right-hand side of the projection."""
+        _chk(lib().b2p_flux_estimator_flux_mult(self.h, _vp(flux_dofs), _vp(rhs)), self.ctx.h)
+
     def project(self, flux_dofs, smooth_dofs):
         _chk(lib().b2p_flux_estimator_project(self.h, _vp(flux_dofs), _vp(smooth_dofs)), self.ctx.h)
 

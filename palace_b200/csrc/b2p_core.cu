@@ -181,6 +181,35 @@ bool op_essential_matches(const b2p_op *op, const int32_t *ess_ldofs, int64_t n)
   if (!op->lidx_bc) return v.empty();
   return op->ess_n == (int64_t)v.size() && op->ess_hash == h;
 }
+
+// Compose the native-order restriction + orientation with the lexicographic->native dof map
+// (restriction.cpp:134-188,281-297) into one signed lexicographic index array.
+int build_lex_restriction(b2p_ctx *ctx, const char *who, const b2p_op_desc *d, int P, int64_t lsize, int ne, int *PS_out, int32_t **out)
+{
+  const int PS = (P + 3) & ~3;
+  *PS_out = PS;
+  std::vector<int32_t> lidx((size_t)ne * PS, (int32_t)B2P_SKIP_IDX);
+  for (int l = 0; l < P; l++)
+  {
+    int nat = d->dof_map ? d->dof_map[l] : l;
+    int sg = 1;
+    if (nat < 0)
+    {
+      nat = -1 - nat;
+      sg = -1;
+    }
+    B2P_CHECK(ctx, nat >= 0 && nat < P, B2P_ERR_ARG, "%sdof_map[%d] out of range", who, l);
+    for (int e = 0; e < ne; e++)
+    {
+      const int32_t gi = d->idx[(size_t)e * P + nat];
+      B2P_CHECK(ctx, gi >= 0 && gi < lsize, B2P_ERR_ARG, "%sidx[%d][%d]=%d outside L-vector of size %lld", who, e, nat, gi,
+                (long long)lsize);
+      const int s = sg * (d->orient ? (int)d->orient[(size_t)e * P + nat] : 1);
+      lidx[(size_t)e * PS + l] = (s >= 0) ? gi : (-1 - gi);
+    }
+  }
+  return upload(ctx, lidx.data(), lidx.size(), out);
+}
 }  // namespace b2p
 
 extern "C"
@@ -510,34 +539,9 @@ int elem_dofs(int kind, int p)
   return 3 * p * (p + 1) * (p + 1);
 }
 
-// Compose the native-order restriction + orientation with the lexicographic->native dof map
-// (restriction.cpp:134-188,281-297) into one signed lexicographic index array.
 int build_restriction(b2p_op *op, const b2p_op_desc *d)
 {
-  const int P = op->P, ne = op->ne;
-  op->PS = (P + 3) & ~3;
-  const int PS = op->PS;
-  std::vector<int32_t> lidx((size_t)ne * PS, (int32_t)B2P_SKIP_IDX);
-  for (int l = 0; l < P; l++)
-  {
-    int nat = d->dof_map ? d->dof_map[l] : l;
-    int sg = 1;
-    if (nat < 0)
-    {
-      nat = -1 - nat;
-      sg = -1;
-    }
-    B2P_CHECK(op->ctx, nat >= 0 && nat < P, B2P_ERR_ARG, "dof_map[%d] out of range", l);
-    for (int e = 0; e < ne; e++)
-    {
-      const int32_t gi = d->idx[(size_t)e * P + nat];
-      B2P_CHECK(op->ctx, gi >= 0 && gi < op->lsize, B2P_ERR_ARG, "idx[%d][%d]=%d outside L-vector of size %lld", e, nat,
-                gi, (long long)op->lsize);
-      const int s = sg * (d->orient ? (int)d->orient[(size_t)e * P + nat] : 1);
-      lidx[(size_t)e * PS + l] = (s >= 0) ? gi : (-1 - gi);
-    }
-  }
-  return upload(op->ctx, lidx.data(), lidx.size(), &op->lidx);
+  return build_lex_restriction(op->ctx, "", d, op->P, op->lsize, op->ne, &op->PS, &op->lidx);
 }
 
 int build_tables(b2p_op *op, const b2p_op_desc *d)

@@ -17,8 +17,11 @@
 // interp[3][Q][P] of reference-space values at the quadrature points and a signed element restriction. These operators run
 // once per solve (post-processing): one CTA per element, dense contractions; they are not on the hot path and make no
 // roofline claim.
+#include <algorithm>
 #include <cmath>
+#include <initializer_list>
 #include <memory>
+#include <utility>
 #include <vector>
 
 #include "b2p_linalg.hpp"
@@ -248,6 +251,20 @@ public:
   const double *d_coef;
 };
 
+// Flux of an estimator on hexahedra (b2p_flux_estimator_create_hex): the sum-factorised mixed mass of b2p_hex_flux.cu
+class HexMixedMassOperator : public Operator
+{
+public:
+  HexMixedMassOperator(b2p_ctx *c, int64_t h, int64_t w, const HexFluxArgs &a_) : Operator(c, h, w), a(a_) {}
+  void Mult(const double *x, double *y) const override
+  {
+    vec::set(ctx, y, height, 0.0);
+    rc = launch_hex_flux_mixed(a, x, y, ctx->stream);
+  }
+  HexFluxArgs a;
+  mutable int rc = B2P_SUCCESS;
+};
+
 // diag[|i|] += sum_q phi_i^T D phi_i (the signs of the restriction cancel)
 __global__ void vecfe_mass_diag_kernel(int ne, int Q, int q1d, VecFESpace sp, const double *__restrict__ qd, const double *__restrict__ coef,
                                        double *diag)
@@ -311,10 +328,11 @@ public:
   double *owned_coef;
 };
 
-int upload_coef(b2p_ctx *ctx, const b2p_geom *geom, int n_attr, const double *coef, double **out)
+// per-element 3x3 blocks [ne][9] from a per-attribute table (identity without one)
+int expand_coef(b2p_ctx *ctx, const b2p_geom *geom, int n_attr, const double *coef, std::vector<double> &c)
 {
   const int ne = geom->ne;
-  std::vector<double> c((size_t)ne * 9, 0.0);
+  c.assign((size_t)ne * 9, 0.0);
   if (!coef)
     for (int el = 0; el < ne; el++) c[(size_t)el * 9] = c[(size_t)el * 9 + 4] = c[(size_t)el * 9 + 8] = 1.0;
   else
@@ -328,7 +346,30 @@ int upload_coef(b2p_ctx *ctx, const b2p_geom *geom, int n_attr, const double *co
       for (int i = 0; i < 9; i++) c[(size_t)el * 9 + i] = coef[(size_t)a * 9 + i];
     }
   }
-  return upload(ctx, c.data(), c.size(), out);
+  return B2P_SUCCESS;
+}
+
+int upload_coef(b2p_ctx *ctx, const b2p_geom *geom, int n_attr, const double *coef, double **out)
+{
+  std::vector<double> c;
+  int rc = expand_coef(ctx, geom, n_attr, coef, c);
+  return rc ? rc : upload(ctx, c.data(), c.size(), out);
+}
+
+// per-element coefficient blocks of the hexahedral kernels: [ne][stride], the k-th table's 3x3 at offset 9 k, zero padding
+int upload_coef_blocks(b2p_ctx *ctx, const b2p_geom *geom, int n_attr, std::initializer_list<const double *> coefs, int stride, double **out)
+{
+  const int ne = geom->ne;
+  std::vector<double> blk((size_t)ne * stride, 0.0), c;
+  int k = 0, rc;
+  for (const double *coef : coefs)
+  {
+    if ((rc = expand_coef(ctx, geom, n_attr, coef, c))) return rc;
+    for (int el = 0; el < ne; el++)
+      for (int i = 0; i < 9; i++) blk[(size_t)el * stride + 9 * k + i] = c[(size_t)el * 9 + i];
+    k++;
+  }
+  return upload(ctx, blk.data(), blk.size(), out);
 }
 
 int upload_space(b2p_ctx *ctx, const b2p_vecfe_space_desc *d, int ne, int Q, VecFESpace *out)
@@ -364,7 +405,13 @@ struct b2p_flux_estimator
   b2p_geom *geom = nullptr;
   VecFESpace flux, smooth;
   double *d_coef_flux = nullptr, *d_coef_disc = nullptr, *d_coef_smooth = nullptr;
-  std::unique_ptr<MixedMassOperator> Flux;
+  std::unique_ptr<Operator> Flux;
+  // b2p_flux_estimator_create_hex: sum-factorised spaces (flux = space a, smooth = space b of both argument sets)
+  bool hex = false;
+  HexFluxArgs hex_err;
+  std::vector<double> h_tab;
+  double *d_tab = nullptr, *d_hex_coef_flux = nullptr, *d_hex_coef_err = nullptr;
+  int32_t *hex_lidx[2] = {nullptr, nullptr};
   const Operator *M = nullptr;
   std::unique_ptr<JacobiSmoother> pc;
   std::unique_ptr<IterativeSolver> pcg;
@@ -384,9 +431,61 @@ struct b2p_flux_estimator
     cudaFree(d_coef_flux);
     cudaFree(d_coef_disc);
     cudaFree(d_coef_smooth);
+    cudaFree(d_tab);
+    cudaFree(d_hex_coef_flux);
+    cudaFree(d_hex_coef_err);
+    cudaFree(hex_lidx[0]);
+    cudaFree(hex_lidx[1]);
     if (geom) b2p_geom_destroy(geom);  // (drops this handle's reference)
   }
 };
+
+namespace
+{
+// ConfigureLinearSolver(use_mg = false) (errorestimator.cpp:63-109), then hand the estimator out
+int finish_estimator(std::unique_ptr<b2p_flux_estimator> &e, const Operator *M, double tol, int max_it, const char *who,
+                     b2p_flux_estimator **out)
+{
+  b2p_ctx *ctx = e->ctx;
+  e->M = M;
+  e->pc = std::make_unique<JacobiSmoother>(ctx, 0.0, 1.0);
+  e->pc->SetOperator(*M);
+  e->pcg = std::make_unique<IterativeSolver>(ctx, KspType::CG);
+  e->pcg->SetInitialGuess(false);
+  e->pcg->rel_tol = tol;
+  e->pcg->abs_tol = 2.220446049250313e-16;
+  e->pcg->max_it = max_it;
+  e->pcg->SetOperator(*M);
+  e->pcg->SetPreconditioner(e->pc.get());
+  e->solver = e->pcg.get();
+  cudaError_t err = cudaPeekAtLastError();
+  B2P_CHECK(ctx, err == cudaSuccess, B2P_ERR_CUDA, "%s: %s", who, cudaGetErrorString(err));
+  *out = e.release();
+  return B2P_SUCCESS;
+}
+
+// restriction and space fields of one validated hexahedral space description (slot 0 = flux, 1 = smooth)
+int hex_space(b2p_flux_estimator *e, const b2p_op_desc *d, int slot, const char *role)
+{
+  b2p_ctx *ctx = e->ctx;
+  const char *W = "b2p_flux_estimator_create_hex";
+  const int ne = e->geom->ne, p = d->p;
+  const int P = d->kind == B2P_ND_MASS ? 3 * p * (p + 1) * (p + 1) : 3 * (p + 1) * p * p;
+  char who[96];
+  snprintf(who, sizeof(who), "%s: %s space: ", W, role);
+  int PS = 0;
+  int rc = build_lex_restriction(ctx, who, d, P, d->lsize, ne, &PS, &e->hex_lidx[slot]);
+  if (rc) return rc;
+  VecFESpace &sp = slot == 0 ? e->flux : e->smooth;
+  sp.P = P;
+  sp.map = d->kind == B2P_ND_MASS ? B2P_MAP_HCURL : B2P_MAP_HDIV;
+  sp.lsize = d->lsize;
+  HexFluxArgs &a = e->hex_err;
+  (slot == 0 ? a.lidx_a : a.lidx_b) = e->hex_lidx[slot];
+  (slot == 0 ? a.PS_a : a.PS_b) = PS;
+  return B2P_SUCCESS;
+}
+}  // namespace
 
 extern "C"
 {
@@ -441,23 +540,105 @@ int b2p_flux_estimator_create(b2p_ctx *ctx, b2p_geom *geom, const b2p_vecfe_spac
   if ((rc = upload_coef(ctx, geom, n_attr, coef_disc, &e->d_coef_disc))) return rc;
   if ((rc = upload_coef(ctx, geom, n_attr, coef_smooth, &e->d_coef_smooth))) return rc;
   e->Flux = std::make_unique<MixedMassOperator>(ctx, geom, e->flux, e->smooth, e->d_coef_flux);
-  e->M = M;
-  // ConfigureLinearSolver(use_mg = false) (errorestimator.cpp:63-109)
-  e->pc = std::make_unique<JacobiSmoother>(ctx, 0.0, 1.0);
-  e->pc->SetOperator(*M);
-  e->pcg = std::make_unique<IterativeSolver>(ctx, KspType::CG);
-  e->pcg->SetInitialGuess(false);
-  e->pcg->rel_tol = tol;
-  e->pcg->abs_tol = 2.220446049250313e-16;
-  e->pcg->max_it = max_it;
-  e->pcg->SetOperator(*M);
-  e->pcg->SetPreconditioner(e->pc.get());
-  e->solver = e->pcg.get();
+  return finish_estimator(e, M, tol, max_it, "b2p_flux_estimator_create", out);
+}
+
+int b2p_flux_estimator_create_hex(b2p_ctx *ctx, b2p_geom *geom, const b2p_op_desc *flux_space, const b2p_op_desc *smooth_space, int n_attr,
+                                  const double *coef_flux, const double *coef_disc, const double *coef_smooth, b2p_operator *smooth_mass,
+                                  double tol, int max_it, b2p_flux_estimator **out)
+{
+  const char *W = "b2p_flux_estimator_create_hex";
+  B2P_CHECK(ctx, ctx && geom && flux_space && smooth_space && out && n_attr > 0 && coef_flux && coef_disc && coef_smooth && smooth_mass,
+            B2P_ERR_ARG, "%s: bad argument", W);
+  B2P_CHECK(ctx, ctx->nranks == 1, B2P_ERR_UNSUPPORTED, "%s: partitioned spaces are not supported yet (T-vectors are taken as L-vectors)",
+            W);
+  // what the descriptions are, before what they ask for
+  for (const auto &[d, role] : {std::pair{flux_space, "flux"}, std::pair{smooth_space, "smooth"}})
+    B2P_CHECK(ctx, d->kind == B2P_ND_MASS || d->kind == B2P_RT_MASS, B2P_ERR_ARG,
+              "%s: the %s space has kind %d; a space is B2P_ND_MASS (Nedelec) or B2P_RT_MASS (Raviart-Thomas)", W, role, d->kind);
+  B2P_CHECK(ctx, flux_space->kind != smooth_space->kind, B2P_ERR_ARG, "%s: both spaces are %s; one Nedelec and one Raviart-Thomas space "
+            "are needed", W, flux_space->kind == B2P_ND_MASS ? "Nedelec" : "Raviart-Thomas");
+  B2P_CHECK(ctx, geom->q1d > 0, B2P_ERR_ARG, "%s: the geometry has no tensor q-data (q1d = 0); use b2p_flux_estimator_create", W);
+  const int p = flux_space->p, q1d = geom->q1d, ne = geom->ne;
+  B2P_CHECK(ctx, smooth_space->p == p, B2P_ERR_ARG, "%s: the flux space has p=%d and the smooth space p=%d; both must be the same", W, p,
+            smooth_space->p);
+  for (const auto &[d, role] : {std::pair{flux_space, "flux"}, std::pair{smooth_space, "smooth"}})
+  {
+    B2P_CHECK(ctx, d->ne == ne, B2P_ERR_ARG, "%s: the %s space has %d elements vs %d in the geometry", W, role, d->ne, ne);
+    B2P_CHECK(ctx, d->idx && d->lsize > 0 && d->Bo && d->Bc, B2P_ERR_ARG, "%s: the %s space lacks its restriction or its Bo / Bc tables", W,
+              role);
+  }
+  Operator *M = operator_of(smooth_mass);
+  B2P_CHECK(ctx, M && M->Height() == smooth_space->lsize && M->Width() == smooth_space->lsize, B2P_ERR_ARG,
+            "%s: the mass operator of the smooth space has the wrong size", W);
+  for (const auto &[d, role] : {std::pair{flux_space, "flux"}, std::pair{smooth_space, "smooth"}})
+    B2P_CHECK(ctx, !d->assemble_qdata, B2P_ERR_UNSUPPORTED, "%s: assembled q-data is not available for the %s space (the flux kernels "
+              "apply their coefficients on the fly)", W, role);
+  B2P_CHECK(ctx, p >= 1 && p <= 6 && p < q1d && q1d <= 7, B2P_ERR_UNSUPPORTED,
+            "%s: unsupported p=%d q1d=%d (hex kernels cover p<=6, p<q1d<=7)", W, p, q1d);
+  // both spaces are evaluated with one pair of 1-D tables: the smooth space's must be the flux space's
+  {
+    const size_t nBo = (size_t)q1d * p, nBc = (size_t)q1d * (p + 1);
+    double scale = 0.0, diff = 0.0;
+    for (size_t i = 0; i < nBo; i++)
+    {
+      scale = std::max(scale, std::fabs(flux_space->Bo[i]));
+      diff = std::max(diff, std::fabs(flux_space->Bo[i] - smooth_space->Bo[i]));
+    }
+    for (size_t i = 0; i < nBc; i++)
+    {
+      scale = std::max(scale, std::fabs(flux_space->Bc[i]));
+      diff = std::max(diff, std::fabs(flux_space->Bc[i] - smooth_space->Bc[i]));
+    }
+    B2P_CHECK(ctx, diff <= 1e-14 * scale, B2P_ERR_ARG,
+              "%s: the smooth space's Bo / Bc tables differ from the flux space's by %.3e; both spaces need the same 1-D tables", W, diff);
+  }
+  auto e = std::make_unique<b2p_flux_estimator>();
+  e->ctx = ctx;
+  geom->refcount++;
+  e->geom = geom;
+  e->hex = true;
+  int rc;
+  if ((rc = hex_space(e.get(), flux_space, 0, "flux")) || (rc = hex_space(e.get(), smooth_space, 1, "smooth"))) return rc;
+  // the 1-D tables (the same for both spaces, checked above), packed as b2p_op packs them: Bo[q1d][p] | Bc[q1d][p+1] | Gc
+  // (not read: zeros)
+  e->h_tab.assign((size_t)q1d * p + 2 * (size_t)q1d * (p + 1), 0.0);
+  std::copy(flux_space->Bo, flux_space->Bo + (size_t)q1d * p, e->h_tab.begin());
+  std::copy(flux_space->Bc, flux_space->Bc + (size_t)q1d * (p + 1), e->h_tab.begin() + (size_t)q1d * p);
+  if ((rc = upload(ctx, e->h_tab.data(), e->h_tab.size(), &e->d_tab))) return rc;
+  if ((rc = upload_coef_blocks(ctx, geom, n_attr, {coef_flux}, 10, &e->d_hex_coef_flux))) return rc;
+  if ((rc = upload_coef_blocks(ctx, geom, n_attr, {coef_disc, coef_smooth}, 18, &e->d_hex_coef_err))) return rc;
+  HexFluxArgs &a = e->hex_err;
+  a.ctx = ctx;
+  a.geom = geom;
+  a.p = p;
+  a.h_tab = e->h_tab.data();
+  a.tab = e->d_tab;
+  a.production = hex_flux_production_eligible(p, q1d, e->h_tab.data());
+  a.space_a = flux_space->kind == B2P_ND_MASS ? 0 : 1;
+  a.ecoef = e->d_hex_coef_err;
+  HexFluxArgs af = a;
+  af.ecoef = e->d_hex_coef_flux;
+  e->Flux = std::make_unique<HexMixedMassOperator>(ctx, smooth_space->lsize, flux_space->lsize, af);
+  return finish_estimator(e, M, tol, max_it, W, out);
+}
+
+// rhs = Flux flux_dofs
+int b2p_flux_estimator_flux_mult(b2p_flux_estimator *e, const double *flux_dofs, double *rhs)
+{
+  if (!e || !flux_dofs || !rhs) return B2P_ERR_ARG;
+  b2p_ctx *ctx = e->ctx;
+  e->Flux->Mult(flux_dofs, rhs);
+  if (e->hex)
+  {
+    const int rc = static_cast<HexMixedMassOperator *>(e->Flux.get())->rc;
+    if (rc) return rc;
+  }
   cudaError_t err = cudaPeekAtLastError();
-  B2P_CHECK(ctx, err == cudaSuccess, B2P_ERR_CUDA, "b2p_flux_estimator_create: %s", cudaGetErrorString(err));
-  *out = e.release();
+  B2P_CHECK(ctx, err == cudaSuccess, B2P_ERR_CUDA, "b2p_flux_estimator_flux_mult: %s", cudaGetErrorString(err));
   return B2P_SUCCESS;
 }
+
 
 // FluxProjector::Mult (errorestimator.cpp:166-175)
 int b2p_flux_estimator_project(b2p_flux_estimator *e, const double *flux_dofs, double *smooth_dofs)
@@ -465,7 +646,8 @@ int b2p_flux_estimator_project(b2p_flux_estimator *e, const double *flux_dofs, d
   if (!e || !flux_dofs || !smooth_dofs) return B2P_ERR_ARG;
   b2p_ctx *ctx = e->ctx;
   if (e->rhs.n != e->smooth.lsize) e->rhs.resize(ctx, e->smooth.lsize);
-  e->Flux->Mult(flux_dofs, e->rhs.p);
+  int rc = b2p_flux_estimator_flux_mult(e, flux_dofs, e->rhs.p);
+  if (rc) return rc;
   e->solver->Mult(e->rhs.p, smooth_dofs);
   if (!e->solver->converged)
     set_error(ctx, "Linear solver did not converge, norm(Ax-b)/norm(b) = %.3e (norm(b) = %.3e)!", e->solver->final_res / e->solver->initial_res,
@@ -483,6 +665,14 @@ int b2p_flux_estimator_integrate(b2p_flux_estimator *e, const double *flux_dofs,
   if (!e || !flux_dofs || !smooth_dofs || !estimates) return B2P_ERR_ARG;
   b2p_ctx *ctx = e->ctx;
   const b2p_geom *g = e->geom;
+  if (e->hex)
+  {
+    const int rc = launch_hex_flux_error(e->hex_err, flux_dofs, smooth_dofs, estimates, ctx->stream);
+    if (rc) return rc;
+    cudaError_t err = cudaPeekAtLastError();
+    B2P_CHECK(ctx, err == cudaSuccess, B2P_ERR_CUDA, "b2p_flux_estimator_integrate: %s", cudaGetErrorString(err));
+    return B2P_SUCCESS;
+  }
   const size_t shmem = (size_t)(e->flux.P + e->smooth.P + 6 * g->Q + FLUX_NT + std::max(e->flux.P, e->smooth.P)) * sizeof(double);
   if (shmem > 48 * 1024) cudaFuncSetAttribute(flux_error_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)shmem);
   B2P_LAUNCH(flux_error_kernel, g->ne, FLUX_NT, shmem, ctx->stream, g->ne, g->Q, g->q1d, e->flux, e->smooth, (const double *)g->qd,

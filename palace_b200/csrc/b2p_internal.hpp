@@ -253,6 +253,30 @@ bool rt_hex_apply7_eligible(b2p_op *op);
 int launch_rt_hex_apply(b2p_op *op, const int32_t *lidx, double alpha, const double *x, double *y, const ApplyRange &rg, cudaStream_t s,
                         bool simple);
 int launch_rt_hex_diag(b2p_op *op, double *diag, cudaStream_t s);
+// Signed lexicographic restriction [ne][*PS] of the b2p_op_desc fields idx / orient / dof_map for P dofs per element (the one
+// restriction builder: b2p_op_create, b2p_op_coarsen and b2p_flux_estimator_create_hex); rows padded to *PS = P rounded up to 4
+// with B2P_SKIP_IDX. `who` prefixes the error messages.
+int build_lex_restriction(b2p_ctx *ctx, const char *who, const b2p_op_desc *d, int P, int64_t lsize, int ne, int *PS, int32_t **lidx);
+// Flux operator and error integrals of the flux estimator on hexahedra (b2p_hex_flux.cu). Space a is the trial space of the mixed
+// mass (the test space is b) or the space of index 1 of the error integral (index 2 is b); space_a: 0 = Nedelec, 1 = Raviart-Thomas.
+struct HexFluxArgs
+{
+  b2p_ctx *ctx = nullptr;
+  const b2p_geom *geom = nullptr;
+  int p = 0;
+  const double *h_tab = nullptr;  // host Bo[q1d][p] | Bc[q1d][p+1] | Gc (zeros), as b2p_op::h_tab (the production kernels' parameter block)
+  const double *tab = nullptr;    // the same on the device
+  bool production = false;        // hex_flux_production_eligible
+  int space_a = 0;
+  const int32_t *lidx_a = nullptr, *lidx_b = nullptr;
+  int PS_a = 0, PS_b = 0;
+  const double *ecoef = nullptr;  // [ne][10] {C, pad} (mixed mass) or [ne][18] {C1, C2} (error integral)
+};
+bool hex_flux_production_eligible(int p, int q1d, const double *h_tab);
+// y_b += Flux x_a
+int launch_hex_flux_mixed(const HexFluxArgs &a, const double *x, double *y, cudaStream_t s);
+// est[e] += int_e |C2 P_b x_b - C1 P_a x_a|^2
+int launch_hex_flux_error(const HexFluxArgs &a, const double *x1, const double *x2, double *est, cudaStream_t s);
 int launch_h1_hex_apply(b2p_op *op, const int32_t *lidx, double alpha, const double *x, double *y, const ApplyRange &rg, cudaStream_t s);
 int launch_h1_hex_apply3(b2p_op *op, const int32_t *lidx, double alpha, const double *x, double *y, const ApplyRange &rg,
                          cudaStream_t s);
