@@ -88,6 +88,8 @@ typedef struct
   int elems_per_batch;  /* elements of one batch */
   int64_t batches;      /* batches of the launch (the last one may be partly filled) */
   int64_t seq;          /* launches recorded on this context so far, this one included */
+  char geom[8];         /* where the geometry came from: "qdata" (stored per-point q-data) or "nodes" (evaluated from the
+                           vertices of a trilinear mesh inside the kernel) */
 } b2p_launch_info;
 /* B2P_ERR_ARG before the first persistent launch on ctx. */
 int b2p_ctx_last_launch(b2p_ctx *ctx, b2p_launch_info *out);

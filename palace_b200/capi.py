@@ -110,16 +110,17 @@ class Ctx:
 class LaunchInfo(C.Structure):
     _fields_ = [
         ("kernel", C.c_char * 48), ("max_grid", C.c_int), ("grid", C.c_int), ("workers", C.c_int), ("elems_per_batch", C.c_int),
-        ("batches", C.c_int64), ("seq", C.c_int64),
+        ("batches", C.c_int64), ("seq", C.c_int64), ("geom", C.c_char * 8),
     ]
 
 
 def last_launch(ctx: Ctx) -> dict:
     """The last persistent element kernel launched on ``ctx`` (b2p_ctx_last_launch): kernel name and form, max_grid (SM count x
-    CTAs per SM), grid, workers per CTA, elems_per_batch, batches and seq (launches recorded so far)."""
+    CTAs per SM), grid, workers per CTA, elems_per_batch, batches, seq (launches recorded so far) and geom, the geometry source
+    ("qdata": stored per-point q-data, "nodes": evaluated from the vertices of a trilinear mesh)."""
     r = LaunchInfo()
     _chk(lib().b2p_ctx_last_launch(ctx.h, C.byref(r)), ctx.h)
-    return {name: (getattr(r, name).decode() if name == "kernel" else int(getattr(r, name))) for name, _ in LaunchInfo._fields_}
+    return {name: (getattr(r, name).decode() if name in ("kernel", "geom") else int(getattr(r, name))) for name, _ in LaunchInfo._fields_}
 
 
 class DenseOpDesc(C.Structure):

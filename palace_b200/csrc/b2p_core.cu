@@ -9,6 +9,7 @@
 
 #include "b2p_internal.hpp"
 #include "b2p_qf.cuh"
+#include "b2p_geom1.cuh"
 
 namespace b2p
 {
@@ -53,8 +54,18 @@ __global__ void geom_hex_kernel(int ne, int k, int q, const double *__restrict__
   if (w >= (size_t)ne * Q) return;
   const int e = (int)(w / Q), iq = (int)(w % Q);
   const int qx = iq % q, qy = (iq / q) % q, qz = iq / (q * q);
-  double J[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
   const double *x = xe + (size_t)e * 3 * Nn;
+  double *o = qd + (size_t)e * 10 * Q + qslot(q, qx, qy, qz);
+  if (k == 1)  // trilinear: the definition the element kernels on node geometry share (b2p_geom1.cuh)
+  {
+    Hex1Line L;
+    hex1_line(x, B + 2 * qy, G + 2 * qy, B + 2 * qz, G + 2 * qz, L);
+    double A[9];
+    hex1_point(L, B + 2 * qx, G + 2 * qx, qw[qx], qw[qy], qw[qz], o[0], A);
+    for (int t = 0; t < 9; t++) o[(1 + t) * Q] = A[t];
+    return;
+  }
+  double J[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
   for (int kk = 0; kk < n; kk++)
     for (int jj = 0; jj < n; jj++)
       for (int ii = 0; ii < n; ii++)
@@ -74,7 +85,6 @@ __global__ void geom_hex_kernel(int ne, int k, int q, const double *__restrict__
   double A[9];
   cofactor33(J, A);
   const double detJ = J[0] * A[0] + J[1] * A[1] + J[2] * A[2];
-  double *o = qd + (size_t)e * 10 * Q + qslot(q, qx, qy, qz);
   o[0] = qw[qx] * qw[qy] * qw[qz] * detJ;
   for (int t = 0; t < 9; t++) o[(1 + t) * Q] = A[t] / detJ;
 }
@@ -95,6 +105,40 @@ int launch_geom_hex(b2p_ctx *ctx, int ne, int k, int q1d, const double *d_xe, co
 
 namespace b2p
 {
+// B2P_ND_KERNEL = 4 | 5 | 6 | 7 forces one of the sum-factorised ND kernels (0: the default routes)
+static int forced_nd_kernel()
+{
+  static const int k = []
+  {
+    const char *e = std::getenv("B2P_ND_KERNEL");
+    return e ? std::atoi(e) : 0;
+  }();
+  return k;
+}
+
+// The nd_hex_apply6_kernel routes of apply_range (the one place that decides them):
+//  * block operators (mixed curl kinds on hexes and sums containing one) at p = 2, 3 unless an apply flag or B2P_ND_KERNEL asks
+//    for another kernel (there is no block form in nd_hex_apply4/5_kernel; B2P_APPLY_CTA_KERNEL / B2P_ND_KERNEL=7 select
+//    nd_hex_apply7_kernel, slower there: DESIGN.md 4.1);
+//  * the symmetric kinds at p = 3 by default, at p = 2 under B2P_ND_KERNEL=6, unless the half-warp kernel, the round-1 kernel or the
+//    CTA kernel is asked for.
+// Each only where nd_hex_apply6_eligible holds (q1d = p + 1, mirror-symmetric tables).
+bool routes_to_nd6(b2p_op *op, int flags)
+{
+  if (op->dense || op->kind == B2P_RT_MASS || op->kind == B2P_H1_DIFFUSION) return false;
+  const int nd_kernel = forced_nd_kernel();
+  if (op->bcoef)
+  {
+    const bool other = (flags & (B2P_APPLY_SIMPLE_KERNEL | B2P_APPLY_ROUND1_KERNEL | B2P_APPLY_HALFWARP_KERNEL)) || nd_kernel == 4 || nd_kernel == 5;
+    const bool cta = (flags & B2P_APPLY_CTA_KERNEL) || nd_kernel == 7;
+    return !other && !cta && nd_hex_apply6_eligible(op);
+  }
+  if (flags & B2P_APPLY_SIMPLE_KERNEL) return false;
+  if (((flags & B2P_APPLY_HALFWARP_KERNEL) || nd_kernel == 5) && nd_hex_apply5_eligible(op)) return false;
+  return (nd_kernel == 6 || (nd_kernel == 0 && op->p == 3)) && !(flags & (B2P_APPLY_ROUND1_KERNEL | B2P_APPLY_CTA_KERNEL)) &&
+         nd_hex_apply6_eligible(op);
+}
+
 int apply_range(b2p_op *op, const int32_t *lidx, double alpha, const double *x, double *y, const ApplyRange &rg, int flags,
                 cudaStream_t s)
 {
@@ -106,21 +150,16 @@ int apply_range(b2p_op *op, const int32_t *lidx, double alpha, const double *x, 
     B2P_CHECK(op->ctx, !rg.xg && !rg.yg, B2P_ERR_UNSUPPORTED, "Raviart-Thomas operators: partitioned applies (ghost pieces) are not supported");
     return launch_rt_hex_apply(op, lidx, alpha, x, y, rg, s, (flags & B2P_APPLY_SIMPLE_KERNEL) != 0);
   }
-  // Block operators (mixed curl kinds on hexes and sums containing one): nd_hex_apply6_kernel (p = 2, 3) or
-  // nd_hex_apply7_kernel (p = 4, 5, 6) at q1d = p + 1 with mirror-symmetric tables, the cross-check kernel for everything else
-  // and whenever an apply flag asks for another kernel (there is no block form in nd_hex_apply4/5_kernel).
-  // B2P_APPLY_CTA_KERNEL / B2P_ND_KERNEL=7 select nd_hex_apply7_kernel at p = 2, 3 too (slower there: DESIGN.md 4.1).
+  const bool nd6 = routes_to_nd6(op, flags);
+  // Block operators: nd_hex_apply6_kernel (routes_to_nd6) or nd_hex_apply7_kernel (p = 4, 5, 6, and p = 2, 3 under
+  // B2P_APPLY_CTA_KERNEL / B2P_ND_KERNEL=7) at q1d = p + 1 with mirror-symmetric tables, the cross-check kernel for everything else
+  // and whenever an apply flag asks for another kernel.
   if (op->bcoef)
   {
     const bool tr = (flags & B2P_APPLY_TRANSPOSE) != 0;
-    static const int forced = []
-    {
-      const char *e = std::getenv("B2P_ND_KERNEL");
-      return e ? std::atoi(e) : 0;
-    }();
+    const int forced = forced_nd_kernel();
     const bool other = (flags & (B2P_APPLY_SIMPLE_KERNEL | B2P_APPLY_ROUND1_KERNEL | B2P_APPLY_HALFWARP_KERNEL)) || forced == 4 || forced == 5;
-    const bool cta = (flags & B2P_APPLY_CTA_KERNEL) || forced == 7;
-    if (!other && !cta && nd_hex_apply6_eligible(op)) return launch_nd_hex_apply6(op, lidx, alpha, x, y, rg, s, tr);
+    if (nd6) return launch_nd_hex_apply6(op, lidx, alpha, x, y, rg, s, tr);
     if (!other && nd_hex_apply7_eligible(op)) return launch_nd_hex_apply7(op, lidx, alpha, x, y, rg, s, tr);
     return launch_nd_hex_apply(op, lidx, alpha, x, y, rg, s, tr);
   }
@@ -129,18 +168,12 @@ int apply_range(b2p_op *op, const int32_t *lidx, double alpha, const double *x, 
   if (simple) return launch_nd_hex_apply(op, lidx, alpha, x, y, rg, s);
   // One-element-per-warp variant (p = 3, q1d = 4, mirror-symmetric tables): opt-in through the apply flag or
   // B2P_ND_KERNEL=5; slower than nd_hex_apply4_kernel (DESIGN.md 4.1), kept for the analysis.
-  // B2P_ND_KERNEL = 4 | 5 | 6 | 7 forces one of the sum-factorised ND kernels; default: the register-gather pipeline
-  // nd_hex_apply6_kernel at p = 3 (q1d = 4), nd_hex_apply7_kernel at p = 2, 4, 5, 6 (q1d = p + 1), each where it measured
-  // faster (DESIGN.md 4.1, tools/nd7_ab.py), nd_hex_apply4_kernel everywhere else.
-  static const int nd_kernel = []
-  {
-    const char *e = std::getenv("B2P_ND_KERNEL");
-    return e ? std::atoi(e) : 0;
-  }();
+  // Default: the register-gather pipeline nd_hex_apply6_kernel at p = 3 (q1d = 4), nd_hex_apply7_kernel at p = 2, 4, 5, 6
+  // (q1d = p + 1), each where it measured faster (DESIGN.md 4.1, tools/nd7_ab.py), nd_hex_apply4_kernel everywhere else.
+  const int nd_kernel = forced_nd_kernel();
   if (((flags & B2P_APPLY_HALFWARP_KERNEL) || nd_kernel == 5) && nd_hex_apply5_eligible(op))
     return launch_nd_hex_apply5(op, lidx, alpha, x, y, rg, s);
-  if ((nd_kernel == 6 || (nd_kernel == 0 && op->p == 3)) && !(flags & (B2P_APPLY_ROUND1_KERNEL | B2P_APPLY_CTA_KERNEL)) &&
-      nd_hex_apply6_eligible(op))
+  if (nd6)
   {
     static const bool trace = std::getenv("B2P_TRACE_KERNEL") != nullptr;
     if (trace) fprintf(stderr, "[b2p] nd_hex_apply6 p=%d q1d=%d kind=%d ne=%d\n", op->p, op->q1d, op->kind, op->ne);
@@ -310,7 +343,15 @@ int b2p_geom_create_hex(b2p_ctx *ctx, int ne, int mesh_order, int q1d, const dou
   B2P_CUDA(ctx, cudaMalloc((void **)&g->qd, (size_t)ne * 10 * Q * sizeof(double)));
   if ((rc = launch_geom_hex(ctx, ne, mesh_order, q1d, d_xe, d_B, d_G, d_qw, g->qd, 0))) return rc;
   B2P_CUDA(ctx, cudaDeviceSynchronize());
-  cudaFree(d_xe);
+  if (mesh_order == 1)
+  {
+    g->xe = d_xe;
+    g->h_nodeB.assign(nodeB, nodeB + (size_t)q1d * n);
+    g->h_nodeG.assign(nodeG, nodeG + (size_t)q1d * n);
+    g->h_qw.assign(qw1d, qw1d + q1d);
+  }
+  else
+    cudaFree(d_xe);
   cudaFree(d_B);
   cudaFree(d_G);
   cudaFree(d_qw);
@@ -390,6 +431,7 @@ void b2p_geom_destroy(b2p_geom *g)
   if (--g->refcount > 0) return;
   cudaFree(g->qd);
   cudaFree(g->attr);
+  cudaFree(g->xe);
   delete g;
 }
 
@@ -892,13 +934,15 @@ int64_t b2p_op_lsize(b2p_op *op) { return op ? op->lsize : 0; }
 int64_t b2p_op_algorithmic_bytes(b2p_op *op)
 {
   if (!op) return 0;
-  // x read once + y written once per unique dof, 4-byte index per element dof, q-data per point.
+  // x read once + y written once per unique dof, 4-byte index per element dof, geometry.
   const int64_t Q = op->geom->Q;
   if (op->dense)  // + the tables once (L2 resident)
     return 16 * op->lsize + (int64_t)op->ne * (4 * (int64_t)op->PS + 80 * Q + 144) + 8 * (int64_t)op->dense_Rpad * op->dense_Ppad;
   const int64_t per_point = op->assembled ? op->aq_ncomp : 10;
+  // q-data, or the 8 vertices (192 bytes) where the element kernel evaluates a trilinear geometry in place
+  const int64_t geom_bytes = (routes_to_nd6(op, 0) && nd_hex_apply6_reads_nodes(op)) ? 192 : 8 * per_point * Q;
   // + per-element coefficient block: 144 bytes (two 3x3 tensors), 288 for block operators (four)
-  return 16 * op->lsize + (int64_t)op->ne * (4 * (int64_t)op->PS + 8 * per_point * Q + (op->assembled ? 0 : (op->bcoef ? 288 : 144)));
+  return 16 * op->lsize + (int64_t)op->ne * (4 * (int64_t)op->PS + geom_bytes + (op->assembled ? 0 : (op->bcoef ? 288 : 144)));
 }
 
 // One operator for a real sum  sum_t c_t A_t  of sum-factorised ND operators over the same geometry, space and essential

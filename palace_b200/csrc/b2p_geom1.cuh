@@ -1,0 +1,72 @@
+// Geometry factors of a trilinear (mesh order 1) hexahedron at a tensor quadrature point, from its 8 vertices: the one definition
+// behind the stored q-data of order-1 meshes (geom_hex_kernel) and the element kernels that evaluate the geometry in place
+// (nd_hex_apply6_kernel on node geometry), so that both routes see the same bits.
+//   x[c * 8 + i + 2 (j + 2 k)]: vertex coordinates (b2p_geom::xe); B[q][2], G[q][2]: the linear nodal basis and its derivative
+//   at the 1-D quadrature points; w: the 1-D quadrature weights.
+// Along a line of fixed (qy, qz) every column of J is a two-term combination in the qx tables: hex1_line forms the 18 line sums
+// once, hex1_point the point -- w detJ and A = adj(J)^T / detJ, as q-data component 0 and components 1 ... 9.
+#pragma once
+#include "b2p_qf.cuh"
+
+namespace b2p
+{
+
+struct Hex1Line
+{
+  double s[3][2], t[3][2], u[3][2];  // [c][i]: sum over (j, k) of x[c][i][j][k] times B_y B_z, G_y B_z, B_y G_z
+};
+
+__device__ __forceinline__ void hex1_line(const double *x, const double By[2], const double Gy[2], const double Bz[2], const double Gz[2],
+                                          Hex1Line &L)
+{
+  double byz[4], gyz[4], bgz[4];  // (j, k) at j + 2 k
+#pragma unroll
+  for (int k = 0; k < 2; k++)
+#pragma unroll
+    for (int j = 0; j < 2; j++)
+    {
+      byz[j + 2 * k] = By[j] * Bz[k];
+      gyz[j + 2 * k] = Gy[j] * Bz[k];
+      bgz[j + 2 * k] = By[j] * Gz[k];
+    }
+#pragma unroll
+  for (int c = 0; c < 3; c++)
+#pragma unroll
+    for (int i = 0; i < 2; i++)
+    {
+      double s = 0.0, t = 0.0, u = 0.0;
+#pragma unroll
+      for (int jk = 0; jk < 4; jk++)
+      {
+        const double v = x[c * 8 + i + 2 * jk];
+        s += byz[jk] * v;
+        t += gyz[jk] * v;
+        u += bgz[jk] * v;
+      }
+      L.s[c][i] = s;
+      L.t[c][i] = t;
+      L.u[c][i] = u;
+    }
+}
+
+// wdetJ = w_x w_y w_z detJ, A = adj(J)^T / detJ (column-major) at point qx of the line
+__device__ __forceinline__ void hex1_point(const Hex1Line &L, const double Bx[2], const double Gx[2], double wx, double wy, double wz,
+                                           double &wdetJ, double A[9])
+{
+  double J[9], adj[9];
+#pragma unroll
+  for (int c = 0; c < 3; c++)
+  {
+    J[c + 0] = Gx[0] * L.s[c][0] + Gx[1] * L.s[c][1];
+    J[c + 3] = Bx[0] * L.t[c][0] + Bx[1] * L.t[c][1];
+    J[c + 6] = Bx[0] * L.u[c][0] + Bx[1] * L.u[c][1];
+  }
+  cofactor33(J, adj);
+  const double detJ = J[0] * adj[0] + J[1] * adj[1] + J[2] * adj[2];
+  const double r = 1.0 / detJ;
+  wdetJ = wx * wy * wz * detJ;
+#pragma unroll
+  for (int t = 0; t < 9; t++) A[t] = adj[t] * r;
+}
+
+}  // namespace b2p

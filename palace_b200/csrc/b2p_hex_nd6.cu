@@ -17,6 +17,10 @@
 //   * XDX can consume the Z region directly (FWD): the y-contraction of the lane's own line is accumulated
 //     straight into the 24 point accumulators, so neither the 25 line inputs nor the forward Y region exist
 // Shared memory per warp drops from 27 KB to ~15 KB and the register budget to <= 168, so 12 warps per SM fit.
+// Node geometry (NODES, the symmetric kinds at p = 3 on a trilinear mesh whose geometry object kept its vertices,
+// b2p_geom::xe; nd_hex_apply6_reads_nodes): no q-data stream at all. The batch's 8 vertices per element (192 B instead of 80 B per point) ride in the ring slot after the
+// coefficient blocks, and the D loop evaluates w detJ and adj(J)^T/detJ at each point from them with the arithmetic of the
+// stored q-data (b2p_geom1.cuh): the staged q-data buffer, its bulk copy and its mbarrier are gone.
 //
 // Reference semantics: ceed::Operator::AddMult over CeedOperatorApplyAdd
 // (/root/reference/palace/fem/libceed/operator.cpp:148-178,192-212); D from
@@ -30,6 +34,7 @@
 #include "b2p_qf.cuh"
 #include "b2p_contract.cuh"
 #include "b2p_pipe.cuh"
+#include "b2p_geom1.cuh"
 
 namespace b2p
 {
@@ -42,6 +47,7 @@ struct ND6Params
 {
   const int32_t *lidx;  // [ne][PS] signed lexicographic restriction, rows padded to 16 bytes (B2P_SKIP_IDX = masked/pad)
   const double *qd;     // [ne][10][Q] geometry, x-slowest point order
+  const double *xe;     // [ne][3][8] element vertices of a trilinear mesh (NODES kernels, instead of qd)
   const double *ecoef;  // [ne][18] per-element coefficient matrices (value part, derivative part)
   const double *x;
   double *y;
@@ -60,6 +66,8 @@ struct ND6Params
   double Bo[H * P_];
   double Bc[H * (P_ + 1)];
   double Gc[H * (P_ + 1)];
+  // NODES: the linear nodal basis, its derivative and the weights at the 1-D points (b2p_geom1.cuh)
+  double nB[2 * Q_], nG[2 * Q_], qw[Q_];
 };
 
 struct Nd6Pad
@@ -92,7 +100,8 @@ constexpr int nd6_lane_stride(int items, int nel)
 // ALIAS: the Y region (written by the second half of XDX, read by Yt) lies on top of the Z region (read by the first
 // half of XDX, written by Yt) -- two extra __syncwarp() separate the reads of one from the writes of the other.
 // GSM: the batch's q-data is staged in shared memory by TMA (as in nd_hex_apply4_kernel) instead of LDG into registers.
-template <int P_, int Q_, int KIND, bool ALIAS = false, bool GSM = false>
+// NODES: no q-data; the batch's element vertices ride in the ring slot after the coefficient blocks.
+template <int P_, int Q_, int KIND, bool ALIAS = false, bool GSM = false, bool NODES = false>
 struct ND6Layout
 {
   static constexpr int p = P_, q = Q_, n = P_ + 1, Q = q * q * q, P = 3 * p * n * n, D3 = p * n * n;
@@ -115,8 +124,11 @@ struct ND6Layout
   static constexpr int LSX = nd6_lane_stride(p * n, NEW), LSZ = nd6_lane_stride(n * n, NEW);
   static constexpr int GE = 10 * Q;   // doubles of q-data per element
   static constexpr int CE = BLOCK ? 36 : 18;  // coefficient doubles per element: two 3x3 tensors, four for the block form
-  // one ring slot: the batch's index rows followed by its coefficient blocks (one mbarrier, one transaction count)
-  static constexpr int SLOT_I = NEW * PS * 4, SLOT_C = NEW * CE * 8, SLOT = (SLOT_I + SLOT_C + 15) & ~15;
+  static constexpr int NE8 = 24;     // doubles of vertex coordinates per element (NODES)
+  // one ring slot: the batch's index rows followed by its coefficient blocks and, with NODES, its vertices (one mbarrier, one
+  // transaction count)
+  static constexpr int SLOT_I = NEW * PS * 4, SLOT_C = NEW * CE * 8, SLOT_N = NODES ? NEW * NE8 * 8 : 0,
+                       SLOT = (SLOT_I + SLOT_C + SLOT_N + 15) & ~15;
   static constexpr int OFF_G = 0;                     // [NEW * GE] doubles of staged q-data (GSM)
   static constexpr int OFF_W = OFF_G + (GSM ? NEW * GE * 8 : 0);
   static constexpr int OFF_R = OFF_W + WTOT * 8;      // [3] ring slots
@@ -171,10 +183,14 @@ __device__ __forceinline__ void scatter_nb(double *y, const VSplit &sp, double *
 
 // GL1 (with GSM = false): L1 is the staging buffer -- the batch's q-data lines are pulled into L1 by prefetch.global.L1 one
 // batch ahead and the LDGs of the D loop hit there (half the L1 data-pipe wavefronts of TMA -> shared -> LDS, no buffer).
-template <int P_, int Q_, int KIND, bool SPLIT, int NW, int MINB, bool FWD, bool GSM = false, bool XLATE = false, bool GL1 = false>
+// NODES (with GSM = GL1 = false): trilinear geometry evaluated at each point from the element's 8 vertices (b2p_geom1.cuh), which
+// arrive with the batch's ring slot -- 192 bytes per element instead of 80 per point of stored q-data.
+template <int P_, int Q_, int KIND, bool SPLIT, int NW, int MINB, bool FWD, bool GSM = false, bool XLATE = false, bool GL1 = false,
+          bool NODES = false>
 __global__ void __launch_bounds__(NW * 32, MINB) nd_hex_apply6_kernel(const __grid_constant__ ND6Params<P_, Q_> prm)
 {
-  using L = ND6Layout<P_, Q_, KIND, FWD, GSM>;
+  static_assert(!NODES || (!GSM && !GL1), "node geometry stages no q-data");
+  using L = ND6Layout<P_, Q_, KIND, FWD, GSM, NODES>;
   constexpr bool ALIAS = FWD;
   static_assert(L::NEW * Q_ * Q_ <= 32, "one XDX item per lane");
   constexpr int p = L::p, q = L::q, n = L::n, Q = L::Q, D3 = L::D3, GE = L::GE, PS = L::PS, NEW = L::NEW, CE = L::CE;
@@ -216,14 +232,16 @@ __global__ void __launch_bounds__(NW * 32, MINB) nd_hex_apply6_kernel(const __gr
   auto issue_ring = [&](int bb, int slot)
   {
     const int e0 = bb * NEW, nel = min(NEW, prm.ne - e0);
-    const uint32_t ib = (uint32_t)(nel * PS * sizeof(int32_t)), cb = (uint32_t)(nel * CE * sizeof(double));
-    mbar_expect_tx(bar_i + slot, ib + cb);
+    const uint32_t ib = (uint32_t)(nel * PS * sizeof(int32_t)), cb = (uint32_t)(nel * CE * sizeof(double)),
+                   nb8 = NODES ? (uint32_t)(nel * L::NE8 * sizeof(double)) : 0u;
+    mbar_expect_tx(bar_i + slot, ib + cb + nb8);
     tma_bulk_g2s_hint(sR + slot * L::SLOT, prm.lidx + (size_t)e0 * PS, ib, bar_i + slot, once);
     tma_bulk_g2s_hint(sR + slot * L::SLOT + L::SLOT_I, prm.ecoef + (size_t)e0 * CE, cb, bar_i + slot, once);
+    if constexpr (NODES) tma_bulk_g2s_hint(sR + slot * L::SLOT + L::SLOT_I + L::SLOT_C, prm.xe + (size_t)e0 * L::NE8, nb8, bar_i + slot, once);
   };
   auto prefetch_geom = [&](int bb)
   {
-    if (GSM || GL1) return;
+    if (GSM || GL1 || NODES) return;
     const int e0 = bb * NEW, nel = min(NEW, prm.ne - e0);
     prefetch_l2_bulk(prm.qd + (size_t)e0 * GE, (uint32_t)(nel * GE * sizeof(double)));
   };
@@ -335,6 +353,7 @@ __global__ void __launch_bounds__(NW * 32, MINB) nd_hex_apply6_kernel(const __gr
     const int e0 = b * NEW, nel = min(NEW, prm.ne - e0);  // nel: valid element slots of this batch
     const int32_t *cI = (const int32_t *)(sR + slot * L::SLOT);
     const double *cC = (const double *)(sR + slot * L::SLOT + L::SLOT_I);
+    const double *cN = (const double *)(sR + slot * L::SLOT + L::SLOT_I + L::SLOT_C);
 
     // ------------------------------------------------------------------ phase Z (z-contraction, from registers)
     {
@@ -501,7 +520,7 @@ __global__ void __launch_bounds__(NW * 32, MINB) nd_hex_apply6_kernel(const __gr
       // q-data of this lane's line, point qx at g[comp * Q + QQ * qx]; rows of a tail batch read element 0 (discarded)
       const double *g = GSM ? sG + (ok ? e : 0) * GE + s : prm.qd + (size_t)(e0 + (ok ? e : 0)) * GE + s;
       double G[2][10];
-      if constexpr (!GSM)
+      if constexpr (!GSM && !NODES)
       {
 #pragma unroll
         for (int c = 0; c < 10; c++) G[0][c] = GL1 ? __ldg(g + c * Q) : ldg_stream_f64(g + c * Q);
@@ -620,10 +639,19 @@ __global__ void __launch_bounds__(NW * 32, MINB) nd_hex_apply6_kernel(const __gr
       }
       if constexpr (ALIAS) __syncwarp();  // every lane has read its Z-region values: the Y region may overwrite them
       const double *C = cC + e * CE;
+      // NODES: this lane's line sums from the element's vertices (broadcast reads); rows of a tail batch read element 0
+      Hex1Line gl;
+      if constexpr (NODES)
+      {
+        const int qy = s % q, qz = s / q;
+        hex1_line(cN + (ok ? e : 0) * L::NE8, prm.nB + 2 * qy, prm.nG + 2 * qy, prm.nB + 2 * qz, prm.nG + 2 * qz, gl);
+      }
 #pragma unroll
       for (int qx = 0; qx < q; qx++)
       {
-        if constexpr (GSM)
+        if constexpr (NODES)
+          hex1_point(gl, prm.nB + 2 * qx, prm.nG + 2 * qx, prm.qw[qx], prm.qw[s % q], prm.qw[s / q], G[qx & 1][0], G[qx & 1] + 1);
+        else if constexpr (GSM)
         {
 #pragma unroll
           for (int c = 0; c < 10; c++) G[qx & 1][c] = g[c * Q + QQ * qx];
@@ -900,17 +928,17 @@ __global__ void __launch_bounds__(NW * 32, MINB) nd_hex_apply6_kernel(const __gr
 #undef TGC
 }
 
-template <int P_, int Q_, int KIND, int NW, int MINB, bool FWD, bool GSM, bool XLATE, bool WITH_SPLIT, bool GL1 = false>
+template <int P_, int Q_, int KIND, int NW, int MINB, bool FWD, bool GSM, bool XLATE, bool WITH_SPLIT, bool GL1 = false, bool NODES = false>
 int launch6_cfg(b2p_op *op, const int32_t *lidx, double alpha, const double *x, double *y, const ApplyRange &rg, cudaStream_t s,
                 bool transpose = false)
 {
-  using L = ND6Layout<P_, Q_, KIND, FWD, GSM>;
+  using L = ND6Layout<P_, Q_, KIND, FWD, GSM, NODES>;
   const size_t shmem = (size_t)NW * L::WS;
   const bool split = rg.xg || rg.yg || (rg.n_owned >= 0 && rg.n_owned < op->lsize);
-  auto kern = nd_hex_apply6_kernel<P_, Q_, KIND, false, NW, MINB, FWD, GSM, XLATE, GL1>;
+  auto kern = nd_hex_apply6_kernel<P_, Q_, KIND, false, NW, MINB, FWD, GSM, XLATE, GL1, NODES>;
   if constexpr (WITH_SPLIT)
   {
-    if (split) kern = nd_hex_apply6_kernel<P_, Q_, KIND, true, NW, MINB, FWD, GSM, XLATE, GL1>;
+    if (split) kern = nd_hex_apply6_kernel<P_, Q_, KIND, true, NW, MINB, FWD, GSM, XLATE, GL1, NODES>;
   }
   else if (split)
   {
@@ -932,6 +960,7 @@ int launch6_cfg(b2p_op *op, const int32_t *lidx, double alpha, const double *x, 
   if (e_cnt <= 0) return B2P_SUCCESS;
   prm.lidx = lidx + (size_t)e_off * op->PS;
   prm.qd = op->geom->qd + (size_t)e_off * 10 * op->geom->Q;
+  prm.xe = NODES ? op->geom->xe + (size_t)e_off * L::NE8 : nullptr;
   if constexpr (L::BLOCK)
     prm.ecoef = (transpose ? op->bcoef_t : op->bcoef) + L::CE * (size_t)e_off;
   else
@@ -954,10 +983,13 @@ int launch6_cfg(b2p_op *op, const int32_t *lidx, double alpha, const double *x, 
   for (int i = 0; i < H * P_; i++) prm.Bo[i] = op->h_tab[i];
   for (int i = 0; i < H * n; i++) prm.Bc[i] = op->h_tab[Q_ * P_ + i];
   for (int i = 0; i < H * n; i++) prm.Gc[i] = op->h_tab[Q_ * P_ + Q_ * n + i];
+  for (int i = 0; i < 2 * Q_; i++) prm.nB[i] = NODES ? op->geom->h_nodeB[i] : 0.0;
+  for (int i = 0; i < 2 * Q_; i++) prm.nG[i] = NODES ? op->geom->h_nodeG[i] : 0.0;
+  for (int i = 0; i < Q_; i++) prm.qw[i] = NODES ? op->geom->h_qw[i] : 0.0;
   const int nb = (e_cnt + L::NEW - 1) / L::NEW;
   int grid = op->ctx->sm_count * MINB;
   if (grid > (nb + NW - 1) / NW) grid = (nb + NW - 1) / NW;
-  record_launch(op->ctx, "nd_hex_apply6_kernel", L::BLOCK, false, op->ctx->sm_count * MINB, grid, NW, L::NEW, nb);
+  record_launch(op->ctx, "nd_hex_apply6_kernel", L::BLOCK, false, op->ctx->sm_count * MINB, grid, NW, L::NEW, nb, NODES);
   if (rg.pdl)
     B2P_LAUNCH_PDL(kern, grid, NW * 32, shmem, s, prm);
   else
@@ -1011,6 +1043,11 @@ int launch6(b2p_op *op, const int32_t *lidx, double alpha, const double *x, doub
     }
   }
 #endif
+  if constexpr (P_ == 3 && KIND != B2P_ND_BLOCK)
+  {
+    if (nd_hex_apply6_reads_nodes(op))  // trilinear mesh: geometry from the vertices, no q-data stream
+      return launch6_cfg<P_, Q_, KIND, ND6_NW, ND6_MINB, ND6_FWD, false, ND6_XLATE, true, false, true>(op, lidx, alpha, x, y, rg, s);
+  }
   return launch6_cfg<P_, Q_, KIND, ND6_NW, ND6_MINB, ND6_FWD, ND6_GSM, ND6_XLATE, true>(op, lidx, alpha, x, y, rg, s, transpose);
 }
 
@@ -1044,6 +1081,11 @@ bool nd_hex_apply6_eligible(b2p_op *op)
   if (op->tab_sym6 < 0) op->tab_sym6 = nd_tables_symmetric(op->h_tab.data(), op->p, op->q1d, 4e-16) ? 1 : 0;
   return op->tab_sym6 == 1;
 }
+
+// Node geometry for the symmetric kinds at p = 3 only. The block form is already at 253-255 registers on the stored q-data and
+// spills with the 18 line sums of the vertex route; at p = 2 the symmetric kinds run on nd_hex_apply7_kernel unless
+// B2P_ND_KERNEL=6 forces this kernel.
+bool nd_hex_apply6_reads_nodes(const b2p_op *op) { return op->geom->xe && op->p == 3 && !op->bcoef; }
 
 int launch_nd_hex_apply6(b2p_op *op, const int32_t *lidx, double alpha, const double *x, double *y, const ApplyRange &rg, cudaStream_t s,
                          bool transpose)

@@ -114,6 +114,11 @@ struct b2p_geom
   int ne = 0, q1d = 0, Q = 0;  // q1d == 0: general (non-tensor) point set in plain order
   double *qd = nullptr;
   int32_t *attr = nullptr;
+  // trilinear meshes (b2p_geom_create_hex with mesh_order 1) only, else null / empty: the element vertices xe[ne][3][8] and the
+  // host copies of the 1-D tables they were expanded with (nodeB[q1d][2], nodeG[q1d][2], qw1d[q1d]), from which a kernel can
+  // evaluate the geometry in place of reading qd (b2p_geom1.cuh)
+  double *xe = nullptr;
+  std::vector<double> h_nodeB, h_nodeG, h_qw;
   int refcount = 1;
 };
 
@@ -207,12 +212,14 @@ inline bool op_nonsymmetric(const b2p_op *op)
 {
   return op->kind == B2P_ND_WEAKCURL || op->kind == B2P_ND_MIXEDCURL || op->bcoef != nullptr;
 }
-// Store the launch record of a persistent element kernel on its context (b2p_ctx_last_launch). `block` / `cplx` name the form.
+// Store the launch record of a persistent element kernel on its context (b2p_ctx_last_launch). `block` / `cplx` name the form,
+// `nodes` says that the kernel evaluated the geometry from the element vertices instead of reading the stored q-data.
 inline void record_launch(b2p_ctx *c, const char *kernel, bool block, bool cplx, int max_grid, int grid, int workers, int elems_per_batch,
-                          int64_t batches)
+                          int64_t batches, bool nodes = false)
 {
   b2p_launch_info &r = c->last_launch;
   snprintf(r.kernel, sizeof(r.kernel), "%s%s%s", kernel, block ? ":block" : "", cplx ? ":cplx" : "");
+  snprintf(r.geom, sizeof(r.geom), "%s", nodes ? "nodes" : "qdata");
   r.max_grid = max_grid;
   r.grid = grid;
   r.workers = workers;
@@ -229,6 +236,11 @@ bool nd_hex_apply5_eligible(b2p_op *op);
 int launch_nd_hex_apply6(b2p_op *op, const int32_t *lidx, double alpha, const double *x, double *y, const ApplyRange &rg, cudaStream_t s,
                          bool transpose = false);
 bool nd_hex_apply6_eligible(b2p_op *op);
+// Does nd_hex_apply6_kernel, when apply_range sends op to it, evaluate the geometry from the vertices of a trilinear mesh (the
+// symmetric kinds at p = 3) instead of reading the stored q-data?
+bool nd_hex_apply6_reads_nodes(const b2p_op *op);
+// Does apply_range send op, with these apply flags, to nd_hex_apply6_kernel?
+bool routes_to_nd6(b2p_op *op, int flags);
 bool nd_tables_symmetric(const double *tab, int p, int q, double rel_tol);
 int launch_nd_hex_apply7(b2p_op *op, const int32_t *lidx, double alpha, const double *x, double *y, const ApplyRange &rg, cudaStream_t s,
                          bool transpose = false);
