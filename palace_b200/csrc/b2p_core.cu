@@ -343,7 +343,11 @@ int b2p_geom_create_hex(b2p_ctx *ctx, int ne, int mesh_order, int q1d, const dou
   B2P_CUDA(ctx, cudaMalloc((void **)&g->qd, (size_t)ne * 10 * Q * sizeof(double)));
   if ((rc = launch_geom_hex(ctx, ne, mesh_order, q1d, d_xe, d_B, d_G, d_qw, g->qd, 0))) return rc;
   B2P_CUDA(ctx, cudaDeviceSynchronize());
-  if (mesh_order == 1)
+  // The vertex route forms the x-derivative column of J once per (qy, qz) line from row 0 of nodeG: keep the vertices only when
+  // the derivative of the linear basis is the same at every 1-D point (exactly so for a Lagrange basis through two nodes).
+  bool g_const = true;
+  for (int c = 0; mesh_order == 1 && c < q1d; c++) g_const = g_const && nodeG[2 * c] == nodeG[0] && nodeG[2 * c + 1] == nodeG[1];
+  if (mesh_order == 1 && g_const)
   {
     g->xe = d_xe;
     g->h_nodeB.assign(nodeB, nodeB + (size_t)q1d * n);

@@ -1,10 +1,12 @@
 // Geometry factors of a trilinear (mesh order 1) hexahedron at a tensor quadrature point, from its 8 vertices: the one definition
-// behind the stored q-data of order-1 meshes (geom_hex_kernel) and the element kernels that evaluate the geometry in place
-// (nd_hex_apply6_kernel on node geometry), so that both routes see the same bits.
+// of J behind the stored q-data of order-1 meshes (geom_hex_kernel) and the element kernels that evaluate the geometry in place
+// (nd_hex_apply6_kernel on node geometry). Both routes form the same J and cof(J); the stored route divides by detJ per entry,
+// the vertex route scales the finished quadrature-point operator once by w / detJ, so the two agree to rounding, not bit for bit.
 //   x[c * 8 + i + 2 (j + 2 k)]: vertex coordinates (b2p_geom::xe); B[q][2], G[q][2]: the linear nodal basis and its derivative
 //   at the 1-D quadrature points; w: the 1-D quadrature weights.
 // Along a line of fixed (qy, qz) every column of J is a two-term combination in the qx tables: hex1_line forms the 18 line sums
-// once, hex1_point the point -- w detJ and A = adj(J)^T / detJ, as q-data component 0 and components 1 ... 9.
+// once, hex1_jacobian J, K = cof(J) = detJ J^-T and detJ at a point, hex1_point the stored q-data on top of it -- w detJ and
+// A = K / detJ, as q-data component 0 and components 1 ... 9.
 #pragma once
 #include "b2p_qf.cuh"
 
@@ -49,11 +51,11 @@ __device__ __forceinline__ void hex1_line(const double *x, const double By[2], c
     }
 }
 
-// wdetJ = w_x w_y w_z detJ, A = adj(J)^T / detJ (column-major) at point qx of the line
-__device__ __forceinline__ void hex1_point(const Hex1Line &L, const double Bx[2], const double Gx[2], double wx, double wy, double wz,
-                                           double &wdetJ, double A[9])
+// J, K = cof(J) = adj(J)^T (column-major) and detJ at point qx of the line. Column 0 (d/dxi_x) depends on qx only through Gx,
+// which is the same at every point for the linear basis.
+__device__ __forceinline__ void hex1_jacobian(const Hex1Line &L, const double Bx[2], const double Gx[2], double J[9], double K[9],
+                                              double &detJ)
 {
-  double J[9], adj[9];
 #pragma unroll
   for (int c = 0; c < 3; c++)
   {
@@ -61,8 +63,16 @@ __device__ __forceinline__ void hex1_point(const Hex1Line &L, const double Bx[2]
     J[c + 3] = Bx[0] * L.t[c][0] + Bx[1] * L.t[c][1];
     J[c + 6] = Bx[0] * L.u[c][0] + Bx[1] * L.u[c][1];
   }
-  cofactor33(J, adj);
-  const double detJ = J[0] * adj[0] + J[1] * adj[1] + J[2] * adj[2];
+  cofactor33(J, K);
+  detJ = J[0] * K[0] + J[1] * K[1] + J[2] * K[2];
+}
+
+// wdetJ = w_x w_y w_z detJ, A = adj(J)^T / detJ (column-major) at point qx of the line
+__device__ __forceinline__ void hex1_point(const Hex1Line &L, const double Bx[2], const double Gx[2], double wx, double wy, double wz,
+                                           double &wdetJ, double A[9])
+{
+  double J[9], adj[9], detJ;
+  hex1_jacobian(L, Bx, Gx, J, adj, detJ);
   const double r = 1.0 / detJ;
   wdetJ = wx * wy * wz * detJ;
 #pragma unroll

@@ -19,8 +19,8 @@
 // Shared memory per warp drops from 27 KB to ~15 KB and the register budget to <= 168, so 12 warps per SM fit.
 // Node geometry (NODES, the symmetric kinds at p = 3 on a trilinear mesh whose geometry object kept its vertices,
 // b2p_geom::xe; nd_hex_apply6_reads_nodes): no q-data stream at all. The batch's 8 vertices per element (192 B instead of 80 B per point) ride in the ring slot after the
-// coefficient blocks, and the D loop evaluates w detJ and adj(J)^T/detJ at each point from them with the arithmetic of the
-// stored q-data (b2p_geom1.cuh): the staged q-data buffer, its bulk copy and its mbarrier are gone.
+// coefficient blocks, and the D loop forms J, cof(J) and detJ at each point from them with the definition of the stored q-data
+// (b2p_geom1.cuh) and applies D scaled once by alpha w / detJ: the staged q-data buffer, its bulk copy and its mbarrier are gone.
 //
 // Reference semantics: ceed::Operator::AddMult over CeedOperatorApplyAdd
 // (/root/reference/palace/fem/libceed/operator.cpp:148-178,192-212); D from
@@ -144,7 +144,19 @@ struct ND6Layout
 inline double ldg_stream_f64(const double *p) { return *p; }
 inline void prefetch_l2_bulk(const void *, uint32_t) {}
 inline void prefetch_l1(const void *) {}
+inline double rcp_f64(double d) { return 1.0 / d; }
 #else
+// 1/d within 1 ulp for normal, non-zero d whose reciprocal is normal, without the slow-path branch of an IEEE division:
+// MUFU.RCP64H and two Newton steps. A degenerate element (detJ = 0) gives inf / NaN, as the division of the stored route does.
+__device__ __forceinline__ double rcp_f64(double d)
+{
+  double r;
+  asm("rcp.approx.ftz.f64 %0, %1;" : "=d"(r) : "d"(d));
+  double e = fma(-d, r, 1.0);
+  r = fma(r, e, r);
+  e = fma(-d, r, 1.0);
+  return fma(r, e, r);
+}
 __device__ __forceinline__ void prefetch_l1(const void *p) { asm volatile("prefetch.global.L1 [%0];" ::"l"(p)); }
 // streaming read: the q-data is used exactly once per launch -- keep it out of L1 (the x gathers reuse lines there)
 __device__ __forceinline__ double ldg_stream_f64(const double *p)
@@ -191,6 +203,7 @@ __global__ void __launch_bounds__(NW * 32, MINB) nd_hex_apply6_kernel(const __gr
 {
   static_assert(!NODES || (!GSM && !GL1), "node geometry stages no q-data");
   using L = ND6Layout<P_, Q_, KIND, FWD, GSM, NODES>;
+  static_assert(!NODES || !L::BLOCK, "the block form runs on stored q-data");
   constexpr bool ALIAS = FWD;
   static_assert(L::NEW * Q_ * Q_ <= 32, "one XDX item per lane");
   constexpr int p = L::p, q = L::q, n = L::n, Q = L::Q, D3 = L::D3, GE = L::GE, PS = L::PS, NEW = L::NEW, CE = L::CE;
@@ -641,17 +654,44 @@ __global__ void __launch_bounds__(NW * 32, MINB) nd_hex_apply6_kernel(const __gr
       const double *C = cC + e * CE;
       // NODES: this lane's line sums from the element's vertices (broadcast reads); rows of a tail batch read element 0
       Hex1Line gl;
+      double wl = 0.0;  // NODES: alpha w_y w_z of the line
       if constexpr (NODES)
       {
         const int qy = s % q, qz = s / q;
         hex1_line(cN + (ok ? e : 0) * L::NE8, prm.nB + 2 * qy, prm.nG + 2 * qy, prm.nB + 2 * qz, prm.nG + 2 * qz, gl);
+        wl = alpha * prm.qw[qy] * prm.qw[qz];
       }
 #pragma unroll
       for (int qx = 0; qx < q; qx++)
       {
         if constexpr (NODES)
-          hex1_point(gl, prm.nB + 2 * qx, prm.nG + 2 * qx, prm.qw[qx], prm.qw[s % q], prm.qw[s / q], G[qx & 1][0], G[qx & 1] + 1);
-        else if constexpr (GSM)
+        {
+          // With K = cof(J) = detJ J^-T and f = alpha w / detJ, the stored route's w detJ A^T C_m A u (A = K / detJ) is
+          // f K^T C_m (K u) and its w detJ Jd^T C_k Jd c (Jd = J / detJ) is f J^T C_k (J c): the four 3x3 products do not wait on
+          // the reciprocal, only the final scaling does. Row 0 of nG serves every qx, so the x-derivative column of J is formed
+          // once per line (the derivative of the linear basis is the same at every point; b2p_geom_create_hex checks it).
+          double J[9], K[9], detJ, v[3] = {0, 0, 0}, cw[3] = {0, 0, 0};
+          hex1_jacobian(gl, prm.nB + 2 * qx, prm.nG, J, K, detJ);
+          const double f = ok ? wl * prm.qw[qx] * rcp_f64(detJ) : 0.0;  // tail slots contribute zero
+          if (prm.iso)
+          {
+            if (MASS) AtAx(K, uu[qx], f * C[0], v);
+            if (CURL) AtAx(J, cc[qx], f * C[9], cw);
+          }
+          else
+          {
+            if (MASS) AtCAx(K, C, uu[qx], f, v);
+            if (CURL) AtCAx(J, C + 9, cc[qx], f, cw);
+          }
+#pragma unroll
+          for (int r = 0; r < 3; r++)
+          {
+            uu[qx][r] = v[r];
+            cc[qx][r] = cw[r];
+          }
+          continue;
+        }
+        if constexpr (GSM)
         {
 #pragma unroll
           for (int c = 0; c < 10; c++) G[qx & 1][c] = g[c * Q + QQ * qx];
@@ -998,16 +1038,17 @@ int launch6_cfg(b2p_op *op, const int32_t *lidx, double alpha, const double *x, 
   return B2P_SUCCESS;
 }
 
-// B2P_ND6_CFG = "<warps per CTA><CTAs per SM><f|y><g|l><e|x>" picks another launch shape / variant of the p = 3
+// B2P_ND6_CFG = "<warps per CTA><CTAs per SM><f|y><g|l|c|n><e|x>" picks another launch shape / variant of the p = 3
 // curl-curl+mass kernel for A/B measurements: f = XDX consumes the Z region, y = separate Y phase; g = q-data staged in
-// shared memory by TMA, l = LDG into registers; e = x gathered right after the Z phase, x = after XDX.
+// shared memory by TMA, l = LDG into registers, c = L1 as the staging buffer, n = geometry from the element vertices (a
+// geometry that kept them only); e = x gathered right after the Z phase, x = after XDX.
 inline int nd6_cfg_code()
 {
   static const int code = []
   {
     const char *e = std::getenv("B2P_ND6_CFG");
     if (!e || std::strlen(e) < 5) return 0;
-    return (e[0] - '0') * 10000 + (e[1] - '0') * 1000 + (e[2] == 'y' ? 100 : 0) + (e[3] == 'g' ? 10 : e[3] == 'c' ? 20 : 0) + (e[4] == 'x' ? 1 : 0);
+    return (e[0] - '0') * 10000 + (e[1] - '0') * 1000 + (e[2] == 'y' ? 100 : 0) + (e[3] == 'g' ? 10 : e[3] == 'c' ? 20 : e[3] == 'n' ? 30 : 0) + (e[4] == 'x' ? 1 : 0);
   }();
   return code;
 }
@@ -1040,6 +1081,12 @@ int launch6(b2p_op *op, const int32_t *lidx, double alpha, const double *x, doub
       case 42021: return launch6_cfg<P_, Q_, KIND, 4, 2, true, false, true, false, true>(op, lidx, alpha, x, y, rg, s);   // "42fcx"
       case 42020: return launch6_cfg<P_, Q_, KIND, 4, 2, true, false, false, false, true>(op, lidx, alpha, x, y, rg, s);  // "42fce"
       case 43021: return launch6_cfg<P_, Q_, KIND, 4, 3, true, false, true, false, true>(op, lidx, alpha, x, y, rg, s);   // "43fcx"
+      case 42031:  // "42fnx"
+        if (nd_hex_apply6_reads_nodes(op)) return launch6_cfg<P_, Q_, KIND, 4, 2, true, false, true, false, false, true>(op, lidx, alpha, x, y, rg, s);
+        break;
+      case 43031:  // "43fnx"
+        if (nd_hex_apply6_reads_nodes(op)) return launch6_cfg<P_, Q_, KIND, 4, 3, true, false, true, false, false, true>(op, lidx, alpha, x, y, rg, s);
+        break;
     }
   }
 #endif
