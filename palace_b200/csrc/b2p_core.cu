@@ -1,4 +1,5 @@
 // Context, errors, device memory helpers, geometry q-data and operator construction for the C ABI.
+#include <cmath>
 #include <cstdlib>
 #include <cstring>
 #include <mutex>
@@ -343,10 +344,12 @@ int b2p_geom_create_hex(b2p_ctx *ctx, int ne, int mesh_order, int q1d, const dou
   B2P_CUDA(ctx, cudaMalloc((void **)&g->qd, (size_t)ne * 10 * Q * sizeof(double)));
   if ((rc = launch_geom_hex(ctx, ne, mesh_order, q1d, d_xe, d_B, d_G, d_qw, g->qd, 0))) return rc;
   B2P_CUDA(ctx, cudaDeviceSynchronize());
-  // The vertex route forms the x-derivative column of J once per (qy, qz) line from row 0 of nodeG: keep the vertices only when
-  // the derivative of the linear basis is the same at every 1-D point (exactly so for a Lagrange basis through two nodes).
-  bool g_const = true;
-  for (int c = 0; mesh_order == 1 && c < q1d; c++) g_const = g_const && nodeG[2 * c] == nodeG[0] && nodeG[2 * c + 1] == nodeG[1];
+  // The vertex route forms the x-derivative column of J once per (qy, qz) line from row 0 of nodeG and the other two columns
+  // with B_0 = 1 - B_1: keep the vertices only when the derivative of the linear basis is the same at every 1-D point and the
+  // basis is a partition of unity (both hold for a Lagrange basis through two nodes).
+  bool g_const = mesh_order == 1;
+  for (int c = 0; g_const && c < q1d; c++)
+    g_const = nodeG[2 * c] == nodeG[0] && nodeG[2 * c + 1] == nodeG[1] && std::fabs(nodeB[2 * c] + nodeB[2 * c + 1] - 1.0) <= 1e-15;
   if (mesh_order == 1 && g_const)
   {
     g->xe = d_xe;

@@ -1,6 +1,6 @@
 // Geometry factors of a trilinear (mesh order 1) hexahedron at a tensor quadrature point, from its 8 vertices: the one definition
 // of J behind the stored q-data of order-1 meshes (geom_hex_kernel) and the element kernels that evaluate the geometry in place
-// (nd_hex_apply6_kernel on node geometry). Both routes form the same J and cof(J); the stored route divides by detJ per entry,
+// (nd_hex_apply6_kernel on node geometry). Both routes form J from the same line sums; the stored route divides by detJ per entry,
 // the vertex route scales the finished quadrature-point operator once by w / detJ, so the two agree to rounding, not bit for bit.
 //   x[c * 8 + i + 2 (j + 2 k)]: vertex coordinates (b2p_geom::xe); B[q][2], G[q][2]: the linear nodal basis and its derivative
 //   at the 1-D quadrature points; w: the 1-D quadrature weights.
@@ -77,6 +77,42 @@ __device__ __forceinline__ void hex1_point(const Hex1Line &L, const double Bx[2]
   wdetJ = wx * wy * wz * detJ;
 #pragma unroll
   for (int t = 0; t < 9; t++) A[t] = adj[t] * r;
+}
+
+// The element kernel's per-point form of the same J. For a Lagrange basis through two nodes B_0 = 1 - B_1, so along the line
+// columns 1 and 2 of J are a + B_1(xi_x) d with a = t[c][0], d = t[c][1] - t[c][0] (u likewise). hex1_kline forms those and
+// column 0 once per line from hex1_line's sums, which it shares with the stored route; hex1_kjacobian then forms J, K = cof(J)
+// and detJ at a point with one FMA per entry of columns 1 and 2 (hex1_jacobian: a product and an FMA). Agrees with
+// hex1_jacobian to rounding.
+struct Hex1KLine
+{
+  double j0[3], a1[3], d1[3], a2[3], d2[3];  // [c]: J[c] = j0, J[c + 3] = a1 + B_1 d1, J[c + 6] = a2 + B_1 d2
+};
+
+__device__ __forceinline__ void hex1_kline(const Hex1Line &L, const double Gx[2], Hex1KLine &K)
+{
+#pragma unroll
+  for (int c = 0; c < 3; c++)
+  {
+    K.j0[c] = Gx[0] * L.s[c][0] + Gx[1] * L.s[c][1];
+    K.a1[c] = L.t[c][0];
+    K.d1[c] = L.t[c][1] - L.t[c][0];
+    K.a2[c] = L.u[c][0];
+    K.d2[c] = L.u[c][1] - L.u[c][0];
+  }
+}
+
+__device__ __forceinline__ void hex1_kjacobian(const Hex1KLine &L, double b1, double J[9], double K[9], double &detJ)
+{
+#pragma unroll
+  for (int c = 0; c < 3; c++)
+  {
+    J[c + 0] = L.j0[c];
+    J[c + 3] = fma(b1, L.d1[c], L.a1[c]);
+    J[c + 6] = fma(b1, L.d2[c], L.a2[c]);
+  }
+  cofactor33(J, K);
+  detJ = J[0] * K[0] + J[1] * K[1] + J[2] * K[2];
 }
 
 }  // namespace b2p

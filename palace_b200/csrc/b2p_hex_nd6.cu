@@ -120,8 +120,21 @@ struct ND6Layout
   static constexpr int Y_X1 = 0, Y_X2 = Y_X1 + (MASS ? NEW * NXA : 0), Y_X3 = Y_X2 + (CURL ? NEW * NXA : 0),
                        Y_Y1 = Y_X3 + (CURL ? NEW * NXA : 0), Y_Y2 = Y_Y1 + NEW * NNA, Y_Z1 = Y_Y2 + (CURL ? NEW * NNA : 0),
                        Y_Z3 = Y_Z1 + NEW * NNA, LY = Y_Z3 + (CURL ? NEW * NNA : 0), RSY = LY + PAD.y;
-  static constexpr int Y0 = ALIAS ? 0 : ZSZ, WEND = (ALIAS && ZSZ > q * RSY) ? ZSZ : Y0 + q * RSY, WTOT = (WEND + 1) & ~1;
   static constexpr int LSX = nd6_lane_stride(p * n, NEW), LSZ = nd6_lane_stride(n * n, NEW);
+  // Z-phase lane rounds and the x values a lane keeps per round
+  static constexpr int LW = (NEW * LSX > NEW * LSZ) ? NEW * LSX : NEW * LSZ;
+  static constexpr int ZROUNDS = (LW + 31) / 32;
+  static constexpr int NXR = 2 * n + p;
+  // Z-phase dump cells: an idle lane of half-warp h (= w / 16) stores its x / y / z-line results from ZD_X / ZD_Y / ZD_Z + 12 h
+  // on instead of into the Z region, so the phase has no divergent region. The cells lie past the Z region, in the Y region or
+  // the tail of the work array, which the Z phase leaves free. Their residues modulo 16 doubles keep them out of every bank an
+  // active lane of the same half-warp stores to, for all p = 2 and p = 3 layouts (the half-warp model of tools/smem_sim.py).
+  static constexpr int ZD_X = ZSZ + ((12 - ZSZ) & 15), ZD_Y = ZSZ + ((3 - ZSZ) & 15), ZD_Z = ZD_Y;
+  static constexpr int ZDH = 12 * (2 * ZROUNDS - 1);
+  static constexpr int ZDX_END = ZD_X + ZDH + (A_XB - A_XA) + q, ZDY_END = ZD_Y + ZDH + (B_YB - B_YA) + q;
+  static constexpr int ZDEND = ZDX_END > ZDY_END ? ZDX_END : ZDY_END;
+  static constexpr int Y0 = ALIAS ? 0 : ZSZ, WEND0 = (ALIAS && ZSZ > q * RSY) ? ZSZ : Y0 + q * RSY,
+                       WEND = WEND0 > ZDEND ? WEND0 : ZDEND, WTOT = (WEND + 1) & ~1;
   static constexpr int GE = 10 * Q;   // doubles of q-data per element
   static constexpr int CE = BLOCK ? 36 : 18;  // coefficient doubles per element: two 3x3 tensors, four for the block form
   static constexpr int NE8 = 24;     // doubles of vertex coordinates per element (NODES)
@@ -134,10 +147,6 @@ struct ND6Layout
   static constexpr int OFF_R = OFF_W + WTOT * 8;      // [3] ring slots
   static constexpr int OFF_B = OFF_R + 3 * SLOT;      // 3 ring mbarriers + 1 for the q-data
   static constexpr int WS = (OFF_B + 4 * 8 + 15) & ~15;
-  // Z-phase lane rounds and the x values a lane keeps per round
-  static constexpr int LW = (NEW * LSX > NEW * LSZ) ? NEW * LSX : NEW * LSZ;
-  static constexpr int ZROUNDS = (LW + 31) / 32;
-  static constexpr int NXR = 2 * n + p;
 };
 
 #ifdef B2P_EMU
@@ -386,10 +395,14 @@ __global__ void __launch_bounds__(NW * 32, MINB) nd_hex_apply6_kernel(const __gr
         }
 #pragma unroll
         for (int k = 0; k < p; k++) uz[k] = signed_x(r, 2 * n + k);
-        // (no divergent regions: idle lanes run on item 0 and their stores are predicated off)
+        // No divergent regions: idle lanes run on item 0 and store into their dump cells (ND6Layout::ZD_*). A predicated store
+        // would let ptxas sink the contractions into a branch region.
+        const int dmp = 12 * (w >> 4);
         {
-          double *xa = sW + L::ZA0 + (tx / p) * RSA + L::A_XA + ex * NXA + q * (tx % p), *xb = xa + (L::A_XB - L::A_XA);
-          double *ya = sW + L::ZB0 + (tx / n) * RSB + L::B_YA + ex * NNA + q * (tx % n), *yb = ya + (L::B_YB - L::B_YA);
+          double *xa = vx ? sW + L::ZA0 + (tx / p) * RSA + L::A_XA + ex * NXA + q * (tx % p) : sW + L::ZD_X + dmp,
+                 *xb = xa + (L::A_XB - L::A_XA);
+          double *ya = vx ? sW + L::ZB0 + (tx / n) * RSB + L::B_YA + ex * NNA + q * (tx % n) : sW + L::ZD_Y + dmp,
+                 *yb = ya + (L::B_YB - L::B_YA);
 #pragma unroll
           for (int qz = 0; qz < q; qz++)
           {
@@ -402,21 +415,21 @@ __global__ void __launch_bounds__(NW * 32, MINB) nd_hex_apply6_kernel(const __gr
               if (CURL) b2 += TGC(qz, k) * ux[k];
               if (CURL) d += TGC(qz, k) * uy[k];
             }
-            if (vx) xa[qz] = a;
-            if (vx) ya[qz] = c;
-            if (CURL && vx) xb[qz] = b2;
-            if (CURL && vx) yb[qz] = d;
+            xa[qz] = a;
+            ya[qz] = c;
+            if (CURL) xb[qz] = b2;
+            if (CURL) yb[qz] = d;
           }
         }
         {
-          double *za = sW + L::ZA0 + (tz / n) * RSA + L::A_ZA + ez * NNA + q * (tz % n);
+          double *za = vz ? sW + L::ZA0 + (tz / n) * RSA + L::A_ZA + ez * NNA + q * (tz % n) : sW + L::ZD_Z + dmp;
 #pragma unroll
           for (int qz = 0; qz < q; qz++)
           {
             double a = 0.0;
 #pragma unroll
             for (int k = 0; k < p; k++) a += TBO(qz, k) * uz[k];
-            if (vz) za[qz] = a;
+            za[qz] = a;
           }
         }
       }
@@ -652,36 +665,104 @@ __global__ void __launch_bounds__(NW * 32, MINB) nd_hex_apply6_kernel(const __gr
       }
       if constexpr (ALIAS) __syncwarp();  // every lane has read its Z-region values: the Y region may overwrite them
       const double *C = cC + e * CE;
-      // NODES: this lane's line sums from the element's vertices (broadcast reads); rows of a tail batch read element 0
-      Hex1Line gl;
-      double wl = 0.0;  // NODES: alpha w_y w_z of the line
+      // NODES: this lane's line constants from the element's vertices (broadcast reads); rows of a tail batch read element 0
+      Hex1KLine gl;
+      double wl = 0.0;  // NODES: alpha w_y w_z of the line, 0 on tail slots
       if constexpr (NODES)
       {
         const int qy = s % q, qz = s / q;
-        hex1_line(cN + (ok ? e : 0) * L::NE8, prm.nB + 2 * qy, prm.nG + 2 * qy, prm.nB + 2 * qz, prm.nG + 2 * qz, gl);
-        wl = alpha * prm.qw[qy] * prm.qw[qz];
+        Hex1Line ls;
+        hex1_line(cN + (ok ? e : 0) * L::NE8, prm.nB + 2 * qy, prm.nG + 2 * qy, prm.nB + 2 * qz, prm.nG + 2 * qz, ls);
+        hex1_kline(ls, prm.nG, gl);  // row 0 of nG serves every qx (b2p_geom_create_hex checks it)
+        wl = (ok ? 1.0 : 0.0) * (alpha * prm.qw[qy] * prm.qw[qz]);  // a 0/1 factor: a select would make ptxas branch around the loads
       }
-#pragma unroll
-      for (int qx = 0; qx < q; qx++)
+      // ISO is warp-uniform (prm.iso): the branch is taken once around the whole point loop, so each copy is one basic block in
+      // which ptxas can interleave the points' dependent chains. A branch per point would split them.
+      auto d_points = [&](auto iso_tag)
       {
-        if constexpr (NODES)
+        [[maybe_unused]] constexpr bool ISO = decltype(iso_tag)::value;  // (the block form has no iso branch)
+#pragma unroll
+        for (int qx = 0; qx < q; qx++)
         {
-          // With K = cof(J) = detJ J^-T and f = alpha w / detJ, the stored route's w detJ A^T C_m A u (A = K / detJ) is
-          // f K^T C_m (K u) and its w detJ Jd^T C_k Jd c (Jd = J / detJ) is f J^T C_k (J c): the four 3x3 products do not wait on
-          // the reciprocal, only the final scaling does. Row 0 of nG serves every qx, so the x-derivative column of J is formed
-          // once per line (the derivative of the linear basis is the same at every point; b2p_geom_create_hex checks it).
-          double J[9], K[9], detJ, v[3] = {0, 0, 0}, cw[3] = {0, 0, 0};
-          hex1_jacobian(gl, prm.nB + 2 * qx, prm.nG, J, K, detJ);
-          const double f = ok ? wl * prm.qw[qx] * rcp_f64(detJ) : 0.0;  // tail slots contribute zero
-          if (prm.iso)
+          if constexpr (NODES)
           {
-            if (MASS) AtAx(K, uu[qx], f * C[0], v);
-            if (CURL) AtAx(J, cc[qx], f * C[9], cw);
+            // With K = cof(J) = detJ J^-T and f = alpha w / detJ, the stored route's w detJ A^T C_m A u (A = K / detJ) is
+            // f K^T C_m (K u) and its w detJ Jd^T C_k Jd c (Jd = J / detJ) is f J^T C_k (J c): the four 3x3 products do not wait
+            // on the reciprocal, only the final scaling does. f is formed on every slot (tail slots hold element 0's geometry)
+            // and zeroed through wl: a select around the reciprocal would make ptxas branch around it.
+            double J[9], K[9], detJ, v[3] = {0, 0, 0}, cw[3] = {0, 0, 0};
+            hex1_kjacobian(gl, prm.nB[2 * qx + 1], J, K, detJ);
+            const double f = wl * prm.qw[qx] * rcp_f64(detJ);
+            if constexpr (ISO)
+            {
+              if (MASS) AtAx(K, uu[qx], f * C[0], v);
+              if (CURL) AtAx(J, cc[qx], f * C[9], cw);
+            }
+            else
+            {
+              if (MASS) AtCAx(K, C, uu[qx], f, v);
+              if (CURL) AtCAx(J, C + 9, cc[qx], f, cw);
+            }
+#pragma unroll
+            for (int r = 0; r < 3; r++)
+            {
+              uu[qx][r] = v[r];
+              cc[qx][r] = cw[r];
+            }
+            continue;
+          }
+          if constexpr (GSM)
+          {
+#pragma unroll
+            for (int c = 0; c < 10; c++) G[qx & 1][c] = g[c * Q + QQ * qx];
+          }
+          else if (qx + 1 < q)
+          {
+            // q-data of the next point of the line is requested before this point's arithmetic
+#pragma unroll
+            for (int c = 0; c < 10; c++) G[(qx + 1) & 1][c] = GL1 ? __ldg(g + c * Q + QQ * (qx + 1)) : ldg_stream_f64(g + c * Q + QQ * (qx + 1));
+          }
+          const double *gq = G[qx & 1];
+          double v[3] = {0, 0, 0}, cw[3] = {0, 0, 0};
+          const double wdetJ = ok ? alpha * gq[0] : 0.0;  // alpha folded into the quadrature weight; tail slots contribute zero
+          const double *A = gq + 1;
+          if constexpr (L::BLOCK)
+          {
+            // out_val = w A^T (Cm A u + Cx Jd c),  out_curl = w Jd^T (Ck Jd c + Cw A u)
+            double Jd[9], t[3], sc[3], a[3], b[3], z[3];
+            cofactor33(A, Jd);
+            Ax33(A, uu[qx], t);
+            Ax33(Jd, cc[qx], sc);
+            Ax33(C, t, a);
+            Ax33(C + 27, sc, b);
+#pragma unroll
+            for (int r = 0; r < 3; r++) z[r] = a[r] + b[r];
+            Atx33(A, z, wdetJ, v);
+            Ax33(C + 9, sc, a);
+            Ax33(C + 18, t, b);
+#pragma unroll
+            for (int r = 0; r < 3; r++) z[r] = a[r] + b[r];
+            Atx33(Jd, z, wdetJ, cw);
+          }
+          else if constexpr (ISO)
+          {
+            if (MASS) AtAx(A, uu[qx], wdetJ * C[0], v);
+            if (CURL)
+            {
+              double Jd[9];
+              cofactor33(A, Jd);
+              AtAx(Jd, cc[qx], wdetJ * C[9], cw);
+            }
           }
           else
           {
-            if (MASS) AtCAx(K, C, uu[qx], f, v);
-            if (CURL) AtCAx(J, C + 9, cc[qx], f, cw);
+            if (MASS) AtCAx(A, C, uu[qx], wdetJ, v);
+            if (CURL)
+            {
+              double Jd[9];
+              cofactor33(A, Jd);
+              AtCAx(Jd, C + 9, cc[qx], wdetJ, cw);
+            }
           }
 #pragma unroll
           for (int r = 0; r < 3; r++)
@@ -689,68 +770,14 @@ __global__ void __launch_bounds__(NW * 32, MINB) nd_hex_apply6_kernel(const __gr
             uu[qx][r] = v[r];
             cc[qx][r] = cw[r];
           }
-          continue;
         }
-        if constexpr (GSM)
-        {
-#pragma unroll
-          for (int c = 0; c < 10; c++) G[qx & 1][c] = g[c * Q + QQ * qx];
-        }
-        else if (qx + 1 < q)
-        {
-          // q-data of the next point of the line is requested before this point's arithmetic
-#pragma unroll
-          for (int c = 0; c < 10; c++) G[(qx + 1) & 1][c] = GL1 ? __ldg(g + c * Q + QQ * (qx + 1)) : ldg_stream_f64(g + c * Q + QQ * (qx + 1));
-        }
-        const double *gq = G[qx & 1];
-        double v[3] = {0, 0, 0}, cw[3] = {0, 0, 0};
-        const double wdetJ = ok ? alpha * gq[0] : 0.0;  // alpha folded into the quadrature weight; tail slots contribute zero
-        const double *A = gq + 1;
-        if constexpr (L::BLOCK)
-        {
-          // out_val = w A^T (Cm A u + Cx Jd c),  out_curl = w Jd^T (Ck Jd c + Cw A u)
-          double Jd[9], t[3], sc[3], a[3], b[3], z[3];
-          cofactor33(A, Jd);
-          Ax33(A, uu[qx], t);
-          Ax33(Jd, cc[qx], sc);
-          Ax33(C, t, a);
-          Ax33(C + 27, sc, b);
-#pragma unroll
-          for (int r = 0; r < 3; r++) z[r] = a[r] + b[r];
-          Atx33(A, z, wdetJ, v);
-          Ax33(C + 9, sc, a);
-          Ax33(C + 18, t, b);
-#pragma unroll
-          for (int r = 0; r < 3; r++) z[r] = a[r] + b[r];
-          Atx33(Jd, z, wdetJ, cw);
-        }
-        else if (prm.iso)
-        {
-          if (MASS) AtAx(A, uu[qx], wdetJ * C[0], v);
-          if (CURL)
-          {
-            double Jd[9];
-            cofactor33(A, Jd);
-            AtAx(Jd, cc[qx], wdetJ * C[9], cw);
-          }
-        }
-        else
-        {
-          if (MASS) AtCAx(A, C, uu[qx], wdetJ, v);
-          if (CURL)
-          {
-            double Jd[9];
-            cofactor33(A, Jd);
-            AtCAx(Jd, C + 9, cc[qx], wdetJ, cw);
-          }
-        }
-#pragma unroll
-        for (int r = 0; r < 3; r++)
-        {
-          uu[qx][r] = v[r];
-          cc[qx][r] = cw[r];
-        }
-      }
+      };
+      if constexpr (L::BLOCK)
+        d_points(std::false_type{});
+      else if (prm.iso)
+        d_points(std::true_type{});
+      else
+        d_points(std::false_type{});
       // transposed x-contraction: outputs formed one at a time
 #pragma unroll
       for (int i = 0; i < p; i++)
