@@ -414,6 +414,31 @@ int b2p_solver_stats(b2p_solver *s, int *its, double *initial_res, double *final
 int b2p_solver_lambda_max(b2p_solver *s, double *out); /* Chebyshev: estimated lambda_max(D^-1 A) * sf_max */
 void b2p_solver_destroy(b2p_solver *s);
 
+/* ---- algebraic coarse solvers (the reference's HypreAmsSolver / BoomerAmgSolver, linalg/{ams,amg}.cpp, GPU configuration) ----
+ * Both take an ASSEMBLED real matrix at set_operator: b2p_operator_csr, the matrix b2p_solver_assembled hands its inner solver,
+ * or the Ar + Ai matrix of b2p_csolver_assembled; anything else (and a partitioned context) fails with B2P_ERR_ARG /
+ * B2P_ERR_UNSUPPORTED. The usual wiring is b2p_solver_assembled(ctx, ams, NULL, &coarse) as the coarse solver of b2p_solver_gmg,
+ * or as coarse_type 2 of b2p_ksp_create / b2p_divfree_create / b2p_flux_estimator_set_multigrid. Setup (aggregation, Galerkin
+ * products, dense pseudo-inverse of the coarsest level) runs on the host at set_operator; a mult runs on the device without
+ * allocation or host synchronisation (CUDA-graph capturable). Both are symmetric and can precondition CG.
+ * b2p_solver_amg: smoothed-aggregation AMG (strength 0.08, three-pass greedy aggregation, one Jacobi-smoothed prolongation, stop
+ *   at <= 500 rows / 10 levels / a level keeping > 80 % of its rows), l1-Jacobi with smooth_it sweeps before and after; mult =
+ *   cycle_it V-cycles from zero, or from the initial guess when set.
+ * b2p_solver_ams: AMS cycle type 14 ("01(3+4+5)10") for the eliminated Nedelec p = 1 matrix: G [n_edges x n_vertices] the discrete
+ *   gradient (host CSR, sorted unique columns, entries +-1), coords[n_vertices][3] the vertex coordinates (host). The auxiliary
+ *   matrices G^T A G and Pi_c^T A Pi_c (Pi_c(e, v) = |G(e, v)| (G x_c)_e / 2) each get an AMG hierarchy with one V-cycle per
+ *   correction; singular != 0 drops the gradient correction (curl-curl without mass, the reference's ams_singular_op). mult =
+ *   exactly cycle_it cycles, no norm checks.
+ * b2p_solver_amg_levels: rows / nnz of each level of hierarchy `hierarchy` (AMG: 0; AMS: 0 = G, 1..3 = Pi_x, Pi_y, Pi_z) of s, of
+ *   the inner solver of a b2p_solver_assembled, or of either as a multigrid's coarse solver; returns the number of levels (0
+ *   for the skipped gradient hierarchy of a singular AMS), -1 if s has no such hierarchy. b2p_solver_amg_setup_ms: host time of
+ *   the last set_operator, -1 likewise. */
+int b2p_solver_amg(b2p_ctx *ctx, int cycle_it, int smooth_it, b2p_solver **out);
+int b2p_solver_ams(b2p_ctx *ctx, int cycle_it, int smooth_it, int singular, int64_t n_edges, int64_t n_vertices,
+                   const int32_t *G_rowptr, const int32_t *G_col, const double *G_val, const double *coords, b2p_solver **out);
+int b2p_solver_amg_levels(b2p_solver *s, int hierarchy, int64_t *rows, int64_t *nnz, int max_levels);
+double b2p_solver_amg_setup_ms(b2p_solver *s);
+
 /* ---- BaseKspSolver: configuration -> Krylov solver + preconditioner (linalg/ksp.cpp:29-102,131-239,256-328) ----
  * The fields mirror config::LinearSolverData (utils/configfile.hpp:1000-1120) with the defaults iodata.cpp:500-545 derives;
  * b2p_ksp_config_default fills them for a solution space of polynomial order `order`. The composer builds

@@ -700,6 +700,42 @@ class Solver:
         lib().b2p_solver_assembled_nnz.restype = C.c_int64
         return int(lib().b2p_solver_assembled_nnz(self.h))
 
+    @classmethod
+    def amg(cls, ctx, cycle_it=1, smooth_it=1):
+        """Smoothed-aggregation AMG on an assembled matrix (set_operator: Operator.from_csr, or wrap it in Solver.assembled)."""
+        h = C.c_void_p()
+        _chk(lib().b2p_solver_amg(ctx.h, int(cycle_it), int(smooth_it), C.byref(h)), ctx.h)
+        return cls(ctx, h)
+
+    @classmethod
+    def ams(cls, ctx, G, coords, cycle_it=1, smooth_it=1, singular=False):
+        """AMS (cycle type 14) for the eliminated ND p = 1 matrix; G: scipy sparse discrete gradient [n_edges x n_vertices] (entries
+        +-1), coords: [n_vertices, 3] vertex coordinates."""
+        import scipy.sparse as sp
+
+        G = sp.csr_matrix(G)
+        G.sum_duplicates()
+        G.sort_indices()
+        rp, col, val = _np(G.indptr, np.int32), _np(G.indices, np.int32), _np(G.data, np.float64)
+        X = _np(coords, np.float64).reshape(-1, 3)
+        h = C.c_void_p()
+        _chk(lib().b2p_solver_ams(ctx.h, int(cycle_it), int(smooth_it), int(bool(singular)), C.c_int64(G.shape[0]), C.c_int64(X.shape[0]),
+                                  _ptr(rp), _ptr(col), _ptr(val), _ptr(X), C.byref(h)), ctx.h)
+        return cls(ctx, h)
+
+    def levels(self, hierarchy=0):
+        """(rows, nnz) per level of an AMG / AMS hierarchy (AMS: 0 = G, 1-3 = Pi_x, Pi_y, Pi_z) of this solver, of the inner solver
+        of Solver.assembled, or of either as a multigrid's coarse solver."""
+        rows, nnz = (C.c_int64 * 16)(), (C.c_int64 * 16)()
+        n = lib().b2p_solver_amg_levels(self.h, int(hierarchy), rows, nnz, 16)
+        if n < 0:
+            raise B2PError(f"b2p_solver_amg_levels: no hierarchy {hierarchy} on this solver")
+        return list(rows[:n]), list(nnz[:n])
+
+    def setup_ms(self):
+        lib().b2p_solver_amg_setup_ms.restype = C.c_double
+        return float(lib().b2p_solver_amg_setup_ms(self.h))
+
     def set_check_interval(self, check_every):
         _chk(lib().b2p_solver_krylov_set_check_interval(self.h, int(check_every)), self.ctx.h)
 

@@ -30,6 +30,12 @@ b2p_operator *wrap_operator(std::unique_ptr<Operator> &&op)  // (handles of oper
   h->op = std::move(op);
   return h;
 }
+b2p_solver *wrap_solver(std::unique_ptr<Solver> &&s)
+{
+  auto *h = new b2p_solver;
+  h->s = std::move(s);
+  return h;
+}
 }  // namespace b2p
 
 #define B2P_TRY(ctx, stmt)                                   \
@@ -145,6 +151,11 @@ public:
   CsrOperator(b2p_ctx *c, b2p_csr *a) : Operator(c, b2p_csr_rows(a), b2p_csr_rows(a)), A(a) {}
   void Mult(const double *x, double *y) const override { b2p_csr_mult(A, x, y, (b2p_stream)ctx->stream); }
   void AssembleDiagonal(double *d) const override { b2p_csr_diag(A, d, (b2p_stream)ctx->stream); }
+  b2p_csr *AssembledMatrix(const double **val) const override
+  {
+    *val = csr_values(A);
+    return A;
+  }
 };
 // A solver that runs on the ASSEMBLED matrix of the ParOperator it is given (MfemWrapperSolver::SetOperator,
 // linalg/solver.cpp:13-30: "Operator is always assembled as a HypreParMatrix"): SetOperator assembles and eliminates the
@@ -183,8 +194,24 @@ public:
     inner->Mult(x, y);
   }
   const b2p_csr *Matrix() const { return csr; }
+  const Solver *Inner() const { return inner.get(); }
+  int Status() const override { return inner->Status(); }
 };
 }  // namespace
+}  // extern "C"
+namespace b2p
+{
+// The solver that runs on the assembled matrix: s itself, the inner solver of a b2p_solver_assembled, and either of them as
+// the coarse solver a multigrid took over.
+const Solver *unwrap_coarse_solver(const Solver *s)
+{
+  if (auto *g = dynamic_cast<const GeometricMultigridSolver *>(s)) s = g->B[0].get();
+  if (auto *a = dynamic_cast<const AssembledSolver *>(s)) s = a->Inner();
+  return s;
+}
+}  // namespace b2p
+extern "C"
+{
 int b2p_operator_csr(b2p_ctx *ctx, b2p_csr *A, b2p_operator **out)
 {
   B2P_CHECK(ctx, ctx && A && out, B2P_ERR_ARG, "b2p_operator_csr: null argument");
@@ -386,7 +413,7 @@ int b2p_solver_set_operator(b2p_solver *s, b2p_operator *A)
 {
   if (!s || !s->s || !A) return B2P_ERR_ARG;
   B2P_TRY(s->s->ctx, s->s->SetOperator(*A->op));
-  return B2P_SUCCESS;
+  return s->s->Status();
 }
 int b2p_solver_set_initial_guess(b2p_solver *s, int flag)
 {

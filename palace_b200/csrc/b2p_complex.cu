@@ -1034,6 +1034,11 @@ public:
   void Mult(const double *x, double *y) const override { csr_mult_values(A, val, x, y, ctx->stream); }
   void MultTranspose(const double *, double *) const override { set_error(ctx, "assembled complex coarse matrix: no transpose"); }
   void AssembleDiagonal(double *d) const override { csr_diag_values(A, val, d, ctx->stream); }
+  b2p_csr *AssembledMatrix(const double **v) const override
+  {
+    *v = val;
+    return A;
+  }
 };
 class CsrBlock2Operator : public Operator
 {
@@ -1191,7 +1196,7 @@ public:
     v2_current = false;
     if (pc) pc->SetOperator(*Ac);
     inner->SetOperator(*Ac);
-    return true;
+    return inner->Status() == B2P_SUCCESS;
   }
   void Mult(CCPtr x, CPtr y) const override
   {

@@ -86,6 +86,9 @@ public:
   // multigrid zeroes them in restricted residuals (gmg.cpp:190-194)
   virtual const int32_t *EssentialTrueDofs() const { return nullptr; }
   virtual int64_t NumEssential() const { return 0; }
+  // Operators that are an assembled real matrix: its CSR pattern and the device values they apply (*val), else nullptr.
+  // The algebraic coarse solvers (b2p_amg.cu) read the matrix through this.
+  virtual b2p_csr *AssembledMatrix(const double **val) const { return nullptr; }
   int64_t Height() const { return height; }
   int64_t Width() const { return width; }
 
@@ -222,6 +225,8 @@ public:
   Solver(b2p_ctx *c) : Operator(c, 0, 0) {}
   virtual void SetOperator(const Operator &op) = 0;
   void SetInitialGuess(bool g) { initial_guess = g; }
+  // Error code of the last SetOperator, for solvers whose setup can refuse the operator they are given
+  virtual int Status() const { return B2P_SUCCESS; }
   // y = y + B (x - A y) style application with a caller-supplied residual work vector
   virtual void Mult2(const double *x, double *y, double *r) const;
   virtual void MultTranspose2(const double *x, double *y, double *r) const { Mult2(x, y, r); }

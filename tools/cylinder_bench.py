@@ -3,7 +3,7 @@
 HEX27 mesh from tests/golden/cylinder_cavity_pec.npz, optionally uniformly refined) through the device stack -- ARPACK
 shift-invert over FGMRES + p-multigrid (LOGARITHMIC coarsening) + Chebyshev/Hiptmair. Reports sizes, setup and solve times,
 operator / V-cycle timings and the eigenfrequencies next to the reference's stored values (level 0) and the closed forms.
-GPU box:  python tools/cylinder_bench.py --order 4 --refine 2 --nev 4      (refine 3 at order 4 = 7.9M dofs)"""
+GPU box:  python tools/cylinder_bench.py --order 4 --refine 2 --nev 4 [--coarse ams]      (refine 3 at order 4 = 7.9M dofs)"""
 import argparse
 import json
 import os
@@ -37,6 +37,9 @@ def main():
     ap.add_argument("--nev", type=int, default=4)
     ap.add_argument("--tol", type=float, default=1e-10)
     ap.add_argument("--coarse-tol", type=float, default=1e-10, help="relative tolerance of the coarse-level PCG (the reference's coarse solve is one AMS V-cycle)")
+    ap.add_argument("--coarse", choices=["pcg", "ams"], default="pcg",
+                    help="coarse solver: Jacobi-PCG to --coarse-tol, or AMS on the assembled p=1 matrix with the reference's defaults "
+                         "(cycle_it = order, mg_cycle_it = 2)")
     ap.add_argument("--cheby-order", type=int, default=0, help="Chebyshev smoother order; 0 = the reference's default max(2p, 4) (iodata.cpp:533-536)")
     args = ap.parse_args()
     import torch
@@ -84,17 +87,30 @@ def main():
         AG[q] = common.gpu_par_operator(ctx, geom, prob, O.H1_DIFFUSION, cf.coeff_ctx(a=sigma), space=h1[q], fine_op=AG[p].local_op)
     G = [common.gpu_interp(ctx, h1[q], nd[q], asm.gradient_comps(q)) for q in orders]
     P = [common.gpu_interp(ctx, nd[a], nd[b], asm.nd_prolongation_comps(a, b)) for a, b in zip(orders[:-1], orders[1:])]
-    coarse = capi.Solver.krylov(ctx, capi.CG, rel_tol=args.coarse_tol, max_it=5000)
-    cj = capi.Solver.jacobi(ctx)
-    coarse.set_check_interval(int(os.environ.get("B2P_COARSE_CG_CHECK", "8")))  # device-resident CG scalars
-    if os.environ.get("B2P_COARSE_ASSEMBLED", "0") == "1":  # PCG on the device-assembled p = 1 matrix (MfemWrapperSolver flow)
-        coarse = capi.Solver.assembled(ctx, coarse, cj)
-    else:
-        cj.set_operator(Pl[orders[0]])
-        coarse.set_preconditioner(cj)
-        coarse.set_operator(Pl[orders[0]])
+    q0 = orders[0]
+
+    def make_coarse():
+        if args.coarse == "ams":
+            # vertex coordinates: the corners of the second-order element nodes (lexicographic, 3 per direction)
+            X = np.zeros((h1[q0].ndofs, 3))
+            for c in range(8):
+                X[np.asarray(m.elems)[:, c]] = np.asarray(m.xe2)[:, :, 2 * (c & 1) + 6 * ((c >> 1) & 1) + 18 * ((c >> 2) & 1)]
+            Gh = common.oracle_interp(h1[q0], nd[q0], hs.discrete_gradient_matrix(1))
+            return capi.Solver.assembled(ctx, capi.Solver.ams(ctx, Gh, X, cycle_it=p)), None
+        c = capi.Solver.krylov(ctx, capi.CG, rel_tol=args.coarse_tol, max_it=5000)
+        cj = capi.Solver.jacobi(ctx)
+        c.set_check_interval(int(os.environ.get("B2P_COARSE_CG_CHECK", "8")))  # device-resident CG scalars
+        if os.environ.get("B2P_COARSE_ASSEMBLED", "0") == "1":  # PCG on the device-assembled p = 1 matrix (MfemWrapperSolver flow)
+            return capi.Solver.assembled(ctx, c, cj), cj
+        cj.set_operator(Pl[q0])
+        c.set_preconditioner(cj)
+        c.set_operator(Pl[q0])
+        return c, cj
+
+    coarse, _cj = make_coarse()
     cheby_order = args.cheby_order if args.cheby_order > 0 else max(2 * p, 4)
-    mg = capi.Solver.gmg(ctx, coarse, P, G, cycle_it=1, smooth_it=1, cheby_order=cheby_order)
+    mg_cycle_it = 2 if args.coarse == "ams" else 1
+    mg = capi.Solver.gmg(ctx, coarse, P, G, cycle_it=mg_cycle_it, smooth_it=1, cheby_order=cheby_order)
     mg.gmg_set_operators([Pl[q] for q in orders], [AG[q] for q in orders])
     ksp = capi.Solver.krylov(ctx, capi.FGMRES, rel_tol=args.tol, max_it=300, max_dim=300)
     ksp.set_operator(A)
@@ -133,15 +149,21 @@ def main():
         level_ms[f"P_p{a}_p{b}"] = timeit(lambda: Pab.mult(va, vb))
     xd.copy_(torch.rand(n, dtype=torch.float64))
     vcycle_ms = timeit(lambda: mg.mult(xd, yd), reps=5)
-    q0 = orders[0]
     c_in = torch.rand(nd[q0].ndofs, dtype=torch.float64, device="cuda")
     c_in[torch.from_numpy(np.asarray(nd[q0].ess_dofs, dtype=np.int64)).cuda()] = 0.0
     c_out = torch.zeros_like(c_in)
-    try:
-        level_ms["coarse_solve"] = timeit(lambda: coarse.mult(c_in, c_out), reps=3)
-        level_ms["coarse_solve_its"] = coarse.stats()["its"]
-    except Exception:
-        pass  # (the assembled coarse solver is owned by the multigrid once handed over)
+    # the multigrid owns its coarse solver: time a second one built the same way on the same level operator
+    solo, _solo_cj = make_coarse()
+    t = time.time()
+    solo.set_operator(Pl[q0])
+    torch.cuda.synchronize()
+    level_ms["coarse_set_operator_ms"] = (time.time() - t) * 1e3
+    level_ms["coarse_solve"] = timeit(lambda: solo.mult(c_in, c_out), reps=3)
+    if args.coarse == "ams":
+        level_ms["coarse_host_setup_ms"] = solo.setup_ms()
+        level_ms["coarse_ams_levels"] = [solo.levels(h)[0] for h in range(4)]
+    elif os.environ.get("B2P_COARSE_ASSEMBLED", "0") != "1":  # (the assembled wrapper keeps no Krylov statistics)
+        level_ms["coarse_solve_its"] = solo.stats()["its"]
     its, t_solve = [], [0.0]
 
     def to_full(v):
@@ -172,8 +194,10 @@ def main():
     t_eig = time.time() - t0
     f = frequencies_ghz(np.sort(lam)).real
     out = {"workload": f"cylinder cavity eigenmodes, ND order {p}, {m.ne} HEX27 elements (refine {args.refine})", "dofs": int(n),
-           "levels": orders, "cheby_order": cheby_order, "coarse_tol": args.coarse_tol,
-           "coarse_level": "Jacobi-PCG on the device-assembled p=1 matrix" if os.environ.get("B2P_COARSE_ASSEMBLED", "0") == "1" else "Jacobi-PCG, matrix-free p=1 operator", "level_dofs": {f"nd_p{q}": int(nd[q].ndofs) for q in orders},
+           "levels": orders, "cheby_order": cheby_order, "coarse_tol": args.coarse_tol, "mg_cycle_it": mg_cycle_it,
+           "coarse_level": (f"AMS (cycle_it {p}) on the device-assembled p=1 matrix" if args.coarse == "ams" else
+                            "Jacobi-PCG on the device-assembled p=1 matrix" if os.environ.get("B2P_COARSE_ASSEMBLED", "0") == "1" else
+                            "Jacobi-PCG, matrix-free p=1 operator"), "level_dofs": {f"nd_p{q}": int(nd[q].ndofs) for q in orders},
            "piece_ms": level_ms, "host_build_s": t_host, "device_setup_s": t_setup, "apply_ms": apply_ms, "apply_MDoF_s": n / apply_ms / 1e3,
            "vcycle_ms": vcycle_ms, "eigensolve_s": t_eig, "linear_solves": len(its), "fgmres_its_per_solve": float(np.mean(its)),
            "time_in_linear_solves_s": t_solve[0], "f_ghz": f.tolist(), "analytic_ghz": analytic_ghz(args.nev).tolist()}
