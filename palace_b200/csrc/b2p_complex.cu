@@ -336,7 +336,8 @@ public:
         // Block sums at q1d = p + 1 with mirror-symmetric tables: one nd_hex_apply7_kernel<..., CPLX> launch reads S_re's and
         // S_im's coefficient blocks (bcoef, or bcoef_t for the Hermitian transpose) instead of 4 applies. S_re / S_im stay:
         // assembly (AssembleValues) reads them, and p = 1 and other tables keep the 4 applies.
-        cta = block && !sum_re->dense && sum_re->bcoef && sum_im->bcoef && nd_hex_apply7_eligible(sum_re);
+        cta = block && !sum_re->dense && sum_re->bcoef && sum_im->bcoef &&
+              choose_hex_complex_kernel(sum_re, (int)terms.size()) == HexComplexKernel::ND7Z;
         fused_imag = !IsReal();
         return;
       }
@@ -345,13 +346,12 @@ public:
       sum_re = sum_im = nullptr;  // not fusable (mixed kinds / spaces): term by term
       return;
     }
-    // p <= 3: nd_hex_apply4_kernel<..., CPLX>; p = 4 ... 6: nd_hex_apply7_kernel<..., CPLX> for sums of two or more terms (a
-    // single term keeps its real applies)
-    const bool cta7 = o0->p >= 4 && terms.size() >= 2;
+    // the one-pass kernel: choose_hex_complex_kernel (a single term at p >= 4 keeps its real applies)
+    const HexComplexKernel zk = choose_hex_complex_kernel(terms[0].op, (int)terms.size());
     for (auto &t : terms)
     {
       b2p_op *o = t.op;
-      if (!(cta7 ? nd_hex_apply7_eligible(o) : nd_hex_apply4z_eligible(o)) || o->bcoef || o->geom != o0->geom || o->p != o0->p ||
+      if (choose_hex_complex_kernel(o, (int)terms.size()) == HexComplexKernel::NONE || o->bcoef || o->geom != o0->geom || o->p != o0->p ||
           o->q1d != o0->q1d || o->ne != o0->ne || o->lsize != o0->lsize || o->PS != o0->PS || !o->ecoef || !o->lidx_bc)
         return;
     }
@@ -369,7 +369,7 @@ public:
       if (cudaMemcpy(fused_e18[i].data(), terms[i].op->ecoef, fused_e18[i].size() * sizeof(double), cudaMemcpyDeviceToHost) != cudaSuccess)
         return;
     fused = fill_fused();
-    cta = fused && cta7;
+    cta = fused && zk == HexComplexKernel::ND7Z;
   }
 
   // zcoef / zcoef_h from the cached per-term material tensors and the current scalar coefficients

@@ -3,7 +3,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <mutex>
-
+#include <set>
 #include <type_traits>
 
 #include <algorithm>
@@ -117,79 +117,133 @@ static int forced_nd_kernel()
   return k;
 }
 
-// The nd_hex_apply6_kernel routes of apply_range (the one place that decides them):
-//  * block operators (mixed curl kinds on hexes and sums containing one) at p = 2, 3 unless an apply flag or B2P_ND_KERNEL asks
-//    for another kernel (there is no block form in nd_hex_apply4/5_kernel; B2P_APPLY_CTA_KERNEL / B2P_ND_KERNEL=7 select
-//    nd_hex_apply7_kernel, slower there: DESIGN.md 4.1);
-//  * the symmetric kinds at p = 3 by default, at p = 2 under B2P_ND_KERNEL=6, unless the half-warp kernel, the round-1 kernel or the
-//    CTA kernel is asked for.
-// Each only where nd_hex_apply6_eligible holds (q1d = p + 1, mirror-symmetric tables).
-bool routes_to_nd6(b2p_op *op, int flags)
+// Largest deviation of the packed 1-D tables (Bo, Bc even, Gc odd about the centre) from mirror symmetry, and largest |entry|.
+static void tables_mirror_deviation(const double *tab, int p, int q, double &dev, double &scale)
 {
-  if (op->dense || op->kind == B2P_RT_MASS || op->kind == B2P_H1_DIFFUSION) return false;
-  const int nd_kernel = forced_nd_kernel();
+  const int n = p + 1;
+  const double *Bo = tab, *Bc = tab + q * p, *Gc = Bc + q * n;
+  scale = 0.0;
+  for (int i = 0; i < q * p + 2 * q * n; i++) scale = std::fmax(scale, std::fabs(tab[i]));
+  dev = 0.0;
+  for (int c = 0; c < q; c++)
+  {
+    for (int i = 0; i < p; i++) dev = std::fmax(dev, std::fabs(Bo[c * p + i] - Bo[(q - 1 - c) * p + (p - 1 - i)]));
+    for (int i = 0; i < n; i++)
+    {
+      dev = std::fmax(dev, std::fabs(Bc[c * n + i] - Bc[(q - 1 - c) * n + (n - 1 - i)]));
+      dev = std::fmax(dev, std::fabs(Gc[c * n + i] + Gc[(q - 1 - c) * n + (n - 1 - i)]));
+    }
+  }
+}
+
+bool nd_tables_symmetric(const double *tab, int p, int q, double rel_tol)
+{
+  double dev, scale;
+  tables_mirror_deviation(tab, p, q, dev, scale);
+  return dev <= rel_tol * scale;
+}
+
+bool nd_tables_symmetric(b2p_op *op, double rel_tol)
+{
+  if (op->tab_dev < 0) tables_mirror_deviation(op->h_tab.data(), op->p, op->q1d, op->tab_dev, op->tab_scale);
+  return op->tab_dev <= rel_tol * op->tab_scale;
+}
+
+// The element kernel of an apply with these flags: the one place that decides it. B2P_ND_KERNEL (`forced` below) and the
+// apply flags SIMPLE, HALFWARP, ROUND1, CTA (B2P_APPLY_*_KERNEL) steer the Nedelec routes; "nd6 / nd5 / nd7" below stand for
+// nd_hex_apply6_eligible / nd_hex_apply5_eligible / nd_hex_apply7_eligible (q1d = p + 1 and mirror-symmetric tables among others).
+//
+//   operator                   condition, first match wins                                         kernel
+//   dense basis                                                                                   DENSE
+//   Raviart-Thomas mass        not SIMPLE and rt_hex_apply7_eligible                              RT7
+//                              otherwise                                                          RT_SIMPLE
+//   block (bcoef)              SIMPLE, ROUND1 or HALFWARP, or forced 4 or 5                       ND_SIMPLE
+//                              neither CTA nor forced 7, and nd6                                  ND6
+//                              nd7                                                                ND7
+//                              otherwise                                                          ND_SIMPLE
+//   H1 diffusion               SIMPLE                                                             H1_SIMPLE
+//                              otherwise                                                          H1V3
+//   symmetric Nedelec kinds    SIMPLE                                                             ND_SIMPLE
+//                              (HALFWARP or forced 5) and nd5                                     ND5
+//                              (forced 6, or unset at p = 3), neither ROUND1 nor CTA, and nd6     ND6
+//                              (CTA, forced 7 or unset), not ROUND1, and nd7                      ND7
+//                              otherwise (forced 6 at p >= 4 included)                            ND4
+//
+// Why these defaults: DESIGN.md 4.1 and tools/nd7_ab.py time nd_hex_apply6_kernel (p = 3, and the block form at p = 2, 3),
+// nd_hex_apply7_kernel (p = 2, 4, 5, 6) and nd_hex_apply4_kernel against each other; nd_hex_apply5_kernel is slower and kept for
+// the analysis. The block form exists only in nd_hex_apply_kernel, nd_hex_apply6_kernel and nd_hex_apply7_kernel.
+HexKernel choose_hex_kernel(b2p_op *op, int flags)
+{
+  if (op->dense) return HexKernel::DENSE;
+  const bool simple = flags & B2P_APPLY_SIMPLE_KERNEL, half = flags & B2P_APPLY_HALFWARP_KERNEL;
+  const bool round1 = flags & B2P_APPLY_ROUND1_KERNEL, cta = flags & B2P_APPLY_CTA_KERNEL;
+  if (op->kind == B2P_RT_MASS) return !simple && rt_hex_apply7_eligible(op) ? HexKernel::RT7 : HexKernel::RT_SIMPLE;
+  const int forced = forced_nd_kernel();
   if (op->bcoef)
   {
-    const bool other = (flags & (B2P_APPLY_SIMPLE_KERNEL | B2P_APPLY_ROUND1_KERNEL | B2P_APPLY_HALFWARP_KERNEL)) || nd_kernel == 4 || nd_kernel == 5;
-    const bool cta = (flags & B2P_APPLY_CTA_KERNEL) || nd_kernel == 7;
-    return !other && !cta && nd_hex_apply6_eligible(op);
+    if (simple || round1 || half || forced == 4 || forced == 5) return HexKernel::ND_SIMPLE;
+    if (!(cta || forced == 7) && nd_hex_apply6_eligible(op)) return HexKernel::ND6;
+    return nd_hex_apply7_eligible(op) ? HexKernel::ND7 : HexKernel::ND_SIMPLE;
   }
-  if (flags & B2P_APPLY_SIMPLE_KERNEL) return false;
-  if (((flags & B2P_APPLY_HALFWARP_KERNEL) || nd_kernel == 5) && nd_hex_apply5_eligible(op)) return false;
-  return (nd_kernel == 6 || (nd_kernel == 0 && op->p == 3)) && !(flags & (B2P_APPLY_ROUND1_KERNEL | B2P_APPLY_CTA_KERNEL)) &&
-         nd_hex_apply6_eligible(op);
+  if (op->kind == B2P_H1_DIFFUSION) return simple ? HexKernel::H1_SIMPLE : HexKernel::H1V3;
+  if (simple) return HexKernel::ND_SIMPLE;
+  if ((half || forced == 5) && nd_hex_apply5_eligible(op)) return HexKernel::ND5;
+  if ((forced == 6 || (forced == 0 && op->p == 3)) && !round1 && !cta && nd_hex_apply6_eligible(op)) return HexKernel::ND6;
+  if ((cta || forced == 7 || forced == 0) && !round1 && nd_hex_apply7_eligible(op)) return HexKernel::ND7;
+  return HexKernel::ND4;
+}
+
+// One pass over the geometry for a complex sum: nd_hex_apply4_kernel<CPLX> at p <= 3 (and for a single term),
+// nd_hex_apply7_kernel<CPLX> for two or more terms at p = 4 ... 6 and for block sums.
+HexComplexKernel choose_hex_complex_kernel(b2p_op *op, int n_terms)
+{
+  if (op->bcoef || (op->p >= 4 && n_terms >= 2)) return nd_hex_apply7_eligible(op) ? HexComplexKernel::ND7Z : HexComplexKernel::NONE;
+  return nd_hex_apply4z_eligible(op) ? HexComplexKernel::ND4Z : HexComplexKernel::NONE;
+}
+
+bool hex_pair_apply_eligible(b2p_op *op)
+{
+  return !op->bcoef && op->kind != B2P_RT_MASS && nd_hex_apply4z_eligible(op) && op->ecoef;
+}
+
+int configure_kernel_once(b2p_ctx *ctx, const void *kern, size_t shmem, int carveout)
+{
+  static std::mutex m;
+  static std::set<std::pair<const void *, int>> done;
+  std::lock_guard<std::mutex> lock(m);
+  if (done.count({kern, ctx->device})) return B2P_SUCCESS;
+  B2P_CUDA(ctx, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)shmem));
+  if (carveout >= 0) B2P_CUDA(ctx, cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, carveout));
+  done.insert({kern, ctx->device});
+  return B2P_SUCCESS;
 }
 
 int apply_range(b2p_op *op, const int32_t *lidx, double alpha, const double *x, double *y, const ApplyRange &rg, int flags,
                 cudaStream_t s)
 {
-  if (op->dense) return launch_dense_apply(op, lidx, alpha, x, y, rg, s, (flags & B2P_APPLY_TRANSPOSE) != 0);
-  // Raviart-Thomas mass (symmetric: the transpose flag changes nothing): rt_hex_apply7_kernel at p = 2 ... 6, q1d = p + 1 with
-  // mirror-symmetric tables, the cross-check kernel for everything else and under B2P_APPLY_SIMPLE_KERNEL. Single partition only.
-  if (op->kind == B2P_RT_MASS)
+  static const bool trace = std::getenv("B2P_TRACE_KERNEL") != nullptr;
+  const bool tr = (flags & B2P_APPLY_TRANSPOSE) != 0;  // the symmetric kinds, H1 and Raviart-Thomas ignore it
+  const HexKernel k = choose_hex_kernel(op, flags);
+  switch (k)
   {
-    B2P_CHECK(op->ctx, !rg.xg && !rg.yg, B2P_ERR_UNSUPPORTED, "Raviart-Thomas operators: partitioned applies (ghost pieces) are not supported");
-    return launch_rt_hex_apply(op, lidx, alpha, x, y, rg, s, (flags & B2P_APPLY_SIMPLE_KERNEL) != 0);
+    case HexKernel::DENSE: return launch_dense_apply(op, lidx, alpha, x, y, rg, s, tr);
+    case HexKernel::RT7:
+    case HexKernel::RT_SIMPLE:
+      B2P_CHECK(op->ctx, !rg.xg && !rg.yg, B2P_ERR_UNSUPPORTED, "Raviart-Thomas operators: partitioned applies (ghost pieces) are not supported");
+      return launch_rt_hex_apply(op, lidx, alpha, x, y, rg, s, k == HexKernel::RT7);
+    case HexKernel::ND_SIMPLE: return launch_nd_hex_apply(op, lidx, alpha, x, y, rg, s, tr);
+    case HexKernel::ND4: return launch_nd_hex_apply4(op, lidx, alpha, x, y, rg, s);
+    case HexKernel::ND5: return launch_nd_hex_apply5(op, lidx, alpha, x, y, rg, s);
+    case HexKernel::ND6:
+      if (trace && !op->bcoef) fprintf(stderr, "[b2p] nd_hex_apply6 p=%d q1d=%d kind=%d ne=%d\n", op->p, op->q1d, op->kind, op->ne);
+      return launch_nd_hex_apply6(op, lidx, alpha, x, y, rg, s, tr);
+    case HexKernel::ND7:
+      if (trace && !op->bcoef) fprintf(stderr, "[b2p] nd_hex_apply7 p=%d q1d=%d kind=%d ne=%d\n", op->p, op->q1d, op->kind, op->ne);
+      return launch_nd_hex_apply7(op, lidx, alpha, x, y, rg, s, tr);
+    case HexKernel::H1_SIMPLE: return launch_h1_hex_apply(op, lidx, alpha, x, y, rg, s);
+    case HexKernel::H1V3: return launch_h1_hex_apply3(op, lidx, alpha, x, y, rg, s);
   }
-  const bool nd6 = routes_to_nd6(op, flags);
-  // Block operators: nd_hex_apply6_kernel (routes_to_nd6) or nd_hex_apply7_kernel (p = 4, 5, 6, and p = 2, 3 under
-  // B2P_APPLY_CTA_KERNEL / B2P_ND_KERNEL=7) at q1d = p + 1 with mirror-symmetric tables, the cross-check kernel for everything else
-  // and whenever an apply flag asks for another kernel.
-  if (op->bcoef)
-  {
-    const bool tr = (flags & B2P_APPLY_TRANSPOSE) != 0;
-    const int forced = forced_nd_kernel();
-    const bool other = (flags & (B2P_APPLY_SIMPLE_KERNEL | B2P_APPLY_ROUND1_KERNEL | B2P_APPLY_HALFWARP_KERNEL)) || forced == 4 || forced == 5;
-    if (nd6) return launch_nd_hex_apply6(op, lidx, alpha, x, y, rg, s, tr);
-    if (!other && nd_hex_apply7_eligible(op)) return launch_nd_hex_apply7(op, lidx, alpha, x, y, rg, s, tr);
-    return launch_nd_hex_apply(op, lidx, alpha, x, y, rg, s, tr);
-  }
-  const bool simple = flags & B2P_APPLY_SIMPLE_KERNEL;
-  if (op->kind == B2P_H1_DIFFUSION) return simple ? launch_h1_hex_apply(op, lidx, alpha, x, y, rg, s) : launch_h1_hex_apply3(op, lidx, alpha, x, y, rg, s);
-  if (simple) return launch_nd_hex_apply(op, lidx, alpha, x, y, rg, s);
-  // One-element-per-warp variant (p = 3, q1d = 4, mirror-symmetric tables): opt-in through the apply flag or
-  // B2P_ND_KERNEL=5; slower than nd_hex_apply4_kernel (DESIGN.md 4.1), kept for the analysis.
-  // Default: the register-gather pipeline nd_hex_apply6_kernel at p = 3 (q1d = 4), nd_hex_apply7_kernel at p = 2, 4, 5, 6
-  // (q1d = p + 1), each where it measured faster (DESIGN.md 4.1, tools/nd7_ab.py), nd_hex_apply4_kernel everywhere else.
-  const int nd_kernel = forced_nd_kernel();
-  if (((flags & B2P_APPLY_HALFWARP_KERNEL) || nd_kernel == 5) && nd_hex_apply5_eligible(op))
-    return launch_nd_hex_apply5(op, lidx, alpha, x, y, rg, s);
-  if (nd6)
-  {
-    static const bool trace = std::getenv("B2P_TRACE_KERNEL") != nullptr;
-    if (trace) fprintf(stderr, "[b2p] nd_hex_apply6 p=%d q1d=%d kind=%d ne=%d\n", op->p, op->q1d, op->kind, op->ne);
-    return launch_nd_hex_apply6(op, lidx, alpha, x, y, rg, s);
-  }
-  // p = 2 ... 6 at q1d = p + 1: nd_hex_apply7_kernel (one CTA per element batch, warps specialised by vector component, one 1-D
-  // line per thread; tools/nd7_ab.py times its shapes against nd_hex_apply4_kernel). B2P_APPLY_CTA_KERNEL / B2P_ND_KERNEL=7 select
-  // it at p = 3 too; B2P_ND_KERNEL=4 or B2P_APPLY_ROUND1_KERNEL select the round-1 kernel.
-  if (((flags & B2P_APPLY_CTA_KERNEL) || nd_kernel == 7 || nd_kernel == 0) && !(flags & B2P_APPLY_ROUND1_KERNEL) && nd_hex_apply7_eligible(op))
-  {
-    static const bool trace = std::getenv("B2P_TRACE_KERNEL") != nullptr;
-    if (trace) fprintf(stderr, "[b2p] nd_hex_apply7 p=%d q1d=%d kind=%d ne=%d\n", op->p, op->q1d, op->kind, op->ne);
-    return launch_nd_hex_apply7(op, lidx, alpha, x, y, rg, s);
-  }
-  return launch_nd_hex_apply4(op, lidx, alpha, x, y, rg, s);
+  return B2P_ERR_UNSUPPORTED;
 }
 }  // namespace b2p
 
@@ -830,7 +884,7 @@ int b2p_op_apply_add_pair(b2p_op *op, double alpha, const double *x0, const doub
     B2P_CHECK(op->ctx, op->lidx_bc, B2P_ERR_ARG, "b2p_op_apply_add_pair: masked apply without b2p_op_set_essential");
     lidx = op->lidx_bc;
   }
-  if (op->bcoef || op->kind == B2P_RT_MASS || !nd_hex_apply4z_eligible(op) || !op->ecoef)
+  if (!hex_pair_apply_eligible(op))
   {
     int rc = b2p::apply_range(op, lidx, alpha, x0, y0, ApplyRange(), flags, (cudaStream_t)s);
     return rc ? rc : b2p::apply_range(op, lidx, alpha, x1, y1, ApplyRange(), flags, (cudaStream_t)s);
@@ -947,7 +1001,7 @@ int64_t b2p_op_algorithmic_bytes(b2p_op *op)
     return 16 * op->lsize + (int64_t)op->ne * (4 * (int64_t)op->PS + 80 * Q + 144) + 8 * (int64_t)op->dense_Rpad * op->dense_Ppad;
   const int64_t per_point = op->assembled ? op->aq_ncomp : 10;
   // q-data, or the 8 vertices (192 bytes) where the element kernel evaluates a trilinear geometry in place
-  const int64_t geom_bytes = (routes_to_nd6(op, 0) && nd_hex_apply6_reads_nodes(op)) ? 192 : 8 * per_point * Q;
+  const int64_t geom_bytes = (choose_hex_kernel(op, 0) == HexKernel::ND6 && nd_hex_apply6_reads_nodes(op)) ? 192 : 8 * per_point * Q;
   // + per-element coefficient block: 144 bytes (two 3x3 tensors), 288 for block operators (four)
   return 16 * op->lsize + (int64_t)op->ne * (4 * (int64_t)op->PS + geom_bytes + (op->assembled ? 0 : (op->bcoef ? 288 : 144)));
 }
@@ -1085,7 +1139,8 @@ int b2p_op_create_sum(b2p_ctx *ctx, int n_terms, b2p_op *const *ops, const doubl
   op->PS = o0->PS;
   op->lsize = o0->lsize;
   op->h_tab = o0->h_tab;
-  op->tab_sym = o0->tab_sym;
+  op->tab_dev = o0->tab_dev;
+  op->tab_scale = o0->tab_scale;
   op->ess_n = o0->ess_n;  // the masked restriction is copied below: same essential set
   op->ess_hash = o0->ess_hash;
   int rc = 0;

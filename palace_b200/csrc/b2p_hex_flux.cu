@@ -537,17 +537,10 @@ int launch_hf_pq(const HexFluxArgs &a, const double *xa, const double *xb, doubl
   using L = HFLayout<P_, Q_, NV>;
   const size_t shmem = (size_t)(Q_ * P_ + Q_ * (P_ + 1) + NEB * L::PER_ELEM) * sizeof(double);
   auto kern = ERR ? flux_hex_error_kernel<P_, Q_, SA, NEB, NT> : flux_hex_mixed_kernel<P_, Q_, SA, NEB, NT>;
-  static bool configured = false;
-  if (!configured)
-  {
-    B2P_CUDA(a.ctx, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)shmem));
-    configured = true;
-  }
-  const int ne = a.geom->ne, grid = (ne + NEB - 1) / NEB;
-  record_launch(a.ctx, ERR ? "flux_hex_error_kernel" : "flux_hex_mixed_kernel", false, false, grid, grid, 1, NEB, grid);
-  B2P_LAUNCH(kern, grid, NT, shmem, s, make_hf_params(a, xa, xb, y, ERR ? 18 : 10));
-  B2P_CUDA(a.ctx, cudaGetLastError());
-  return B2P_SUCCESS;
+  if (int rc = configure_kernel(a.ctx, kern, shmem)) return rc;
+  const int grid = (a.geom->ne + NEB - 1) / NEB;  // one CTA per batch
+  return launch_persistent(kern, make_hf_params(a, xa, xb, y, ERR ? 18 : 10), NT, shmem, s, false, a.ctx,
+                           ERR ? "flux_hex_error_kernel" : "flux_hex_mixed_kernel", false, false, grid, 1, NEB, grid);
 }
 
 template <int P_, int SA, bool ERR>
@@ -558,12 +551,7 @@ int launch_hf7(const HexFluxArgs &a, const double *xa, const double *xb, double 
   using L = HF7Layout<P_, S::NE, NV>;
   constexpr int NT = 3 * S::WPC * 32;
   auto kern = ERR ? flux_hex_error7_kernel<P_, SA, S::NE, S::WPC, S::MINB_E> : flux_hex_mixed7_kernel<P_, SA, S::NE, S::WPC, S::MINB>;
-  static bool configured = false;
-  if (!configured)
-  {
-    B2P_CUDA(a.ctx, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)L::SMEM_BYTES));
-    configured = true;
-  }
+  if (int rc = configure_kernel(a.ctx, kern, L::SMEM_BYTES)) return rc;
   HF7Params<P_> prm;
   prm.lidx_a = a.lidx_a;
   prm.lidx_b = a.lidx_b;
@@ -576,14 +564,10 @@ int launch_hf7(const HexFluxArgs &a, const double *xa, const double *xb, double 
   prm.y = y;
   prm.sink = a.ctx->d_sink;
   prm.ne = a.geom->ne;
-  constexpr int q = P_ + 1, n = P_ + 1;
-  for (int i = 0; i < q * P_; i++) prm.Bo[i] = a.h_tab[i];
-  for (int i = 0; i < q * n; i++) prm.Bc[i] = a.h_tab[q * P_ + i];
-  const int grid = (prm.ne + S::NE - 1) / S::NE;
-  record_launch(a.ctx, ERR ? "flux_hex_error7_kernel" : "flux_hex_mixed7_kernel", false, false, grid, grid, 1, S::NE, grid);
-  B2P_LAUNCH(kern, grid, NT, L::SMEM_BYTES, s, prm);
-  B2P_CUDA(a.ctx, cudaGetLastError());
-  return B2P_SUCCESS;
+  copy_tables(a.h_tab, P_, P_ + 1, P_ + 1, prm.Bo, prm.Bc, nullptr);
+  const int grid = (prm.ne + S::NE - 1) / S::NE;  // one CTA per batch
+  return launch_persistent(kern, prm, NT, L::SMEM_BYTES, s, false, a.ctx, ERR ? "flux_hex_error7_kernel" : "flux_hex_mixed7_kernel", false,
+                           false, grid, 1, S::NE, grid);
 }
 
 template <bool ERR>

@@ -199,14 +199,9 @@ int launch_pq(b2p_op *op, const int32_t *lidx, double alpha, const double *x, do
   constexpr int NT = 256;
   const size_t shmem = (size_t)(2 * Q_ * (P_ + 1) + NEB * L::PER_ELEM) * sizeof(double);
   auto kern = h1_hex_diffusion_kernel<P_, Q_, ASM, NEB, NT>;
-  static bool configured = false;
-  if (!configured)
-  {
-    B2P_CUDA(op->ctx, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)shmem));
-    configured = true;
-  }
-  const int ne_run = rg.e_cnt < 0 ? op->ne - rg.e_off : rg.e_cnt;
+  const int ne_run = range_count(op, rg);
   if (ne_run <= 0) return B2P_SUCCESS;
+  if (int rc = configure_kernel(op->ctx, kern, shmem)) return rc;
   B2P_LAUNCH(kern, (ne_run + NEB - 1) / NEB, NT, shmem, s, make_params(op, lidx, alpha, x, y, rg));
   B2P_CUDA(op->ctx, cudaGetLastError());
   return B2P_SUCCESS;

@@ -409,17 +409,12 @@ int launch_h1v3(b2p_op *op, const int32_t *lidx, double alpha, const double *x, 
   constexpr int MINB = (WPS >= 12) ? 3 : (WPS >= 8) ? 2 : 1;
   constexpr int NW = (WPS / MINB) < 1 ? 1 : WPS / MINB;
   const size_t shmem = (size_t)NW * L::WS;
-  const bool split = rg.xg || rg.yg || (rg.n_owned >= 0 && rg.n_owned < op->lsize);
+  const bool split = range_split(op, rg);
   auto kern = split ? h1_hex_apply3_kernel<P_, Q_, ASM, true, NW, MINB> : h1_hex_apply3_kernel<P_, Q_, ASM, false, NW, MINB>;
-  static bool configured[2] = {false, false};
-  if (!configured[split])
-  {
-    B2P_CUDA(op->ctx, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)shmem));
-    configured[split] = true;
-  }
-  H1V3Params<P_, Q_> prm;
-  const int e_off = rg.e_off, e_cnt = rg.e_cnt < 0 ? op->ne - rg.e_off : rg.e_cnt;
+  const int e_off = rg.e_off, e_cnt = range_count(op, rg);
   if (e_cnt <= 0) return B2P_SUCCESS;
+  if (int rc = configure_kernel(op->ctx, kern, shmem)) return rc;
+  H1V3Params<P_, Q_> prm;
   prm.lidx = lidx + (size_t)e_off * op->PS;
   prm.qd = op->geom->qd + (size_t)e_off * 10 * op->geom->Q;
   prm.aq = op->aq ? op->aq + (size_t)e_off * op->aq_estride : nullptr;
@@ -428,19 +423,11 @@ int launch_h1v3(b2p_op *op, const int32_t *lidx, double alpha, const double *x, 
   prm.y = y;
   prm.alpha = alpha;
   prm.ne = e_cnt;
-  prm.sp.n_owned = rg.n_owned < 0 ? op->lsize : rg.n_owned;
-  prm.sp.xg = rg.xg;
-  prm.sp.yg = rg.yg;
-  const int n = P_ + 1;
-  for (int i = 0; i < Q_ * n; i++) prm.Bc[i] = op->h_tab[Q_ * P_ + i];
-  for (int i = 0; i < Q_ * n; i++) prm.Gc[i] = op->h_tab[Q_ * P_ + Q_ * n + i];
+  set_split(prm, op, rg);
+  copy_tables(op->h_tab.data(), P_, Q_, Q_, nullptr, prm.Bc, prm.Gc);
   const int nb = (e_cnt + L::NEW - 1) / L::NEW;
-  int grid = op->ctx->sm_count * MINB;
-  if (grid > (nb + NW - 1) / NW) grid = (nb + NW - 1) / NW;
-  record_launch(op->ctx, "h1_hex_apply3_kernel", false, false, op->ctx->sm_count * MINB, grid, NW, L::NEW, nb);
-  B2P_LAUNCH(kern, grid, NW * 32, shmem, s, prm);
-  B2P_CUDA(op->ctx, cudaGetLastError());
-  return B2P_SUCCESS;
+  return launch_persistent(kern, prm, NW * 32, shmem, s, false, op->ctx, "h1_hex_apply3_kernel", false, false, op->ctx->sm_count * MINB, NW,
+                           L::NEW, nb);
 }
 
 }  // namespace

@@ -889,27 +889,17 @@ int launch4(b2p_op *op, const int32_t *lidx, double alpha, const double *x, doub
   constexpr int NW = (WPS / MINB) < 1 ? 1 : WPS / MINB;
   const size_t shmem = (size_t)NW * L::WS;
   // SPLIT: the L-vector comes in two pieces (owned part in x / y, ghosts in separate buffers)
-  const bool split = rg.xg || rg.yg || (rg.n_owned >= 0 && rg.n_owned < op->lsize);
+  const bool split = range_split(op, rg);
   auto kern = split ? nd_hex_apply4_kernel<P_, Q_, KIND, ASM, true, NW, MINB> : nd_hex_apply4_kernel<P_, Q_, KIND, ASM, false, NW, MINB>;
-  int variant = split ? 1 : 0;
   if constexpr (!ASM && Q_ == P_ + 1)
   {
     static const bool fwd = []() { const char *e = std::getenv("B2P_ND_FWDCHAIN"); return e && e[0] == '1'; }();
-    if (fwd && !split)
-    {
-      kern = nd_hex_apply4_kernel<P_, Q_, KIND, ASM, false, NW, MINB, false, true>;
-      variant = 2;
-    }
+    if (fwd && !split) kern = nd_hex_apply4_kernel<P_, Q_, KIND, ASM, false, NW, MINB, false, true>;
   }
-  static bool configured[3] = {false, false, false};
-  if (!configured[variant])
-  {
-    B2P_CUDA(op->ctx, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)shmem));
-    configured[variant] = true;
-  }
-  ND4Params<P_, Q_> prm;
-  const int e_off = rg.e_off, e_cnt = rg.e_cnt < 0 ? op->ne - rg.e_off : rg.e_cnt;
+  const int e_off = rg.e_off, e_cnt = range_count(op, rg);
   if (e_cnt <= 0) return B2P_SUCCESS;
+  if (int rc = configure_kernel(op->ctx, kern, shmem)) return rc;
+  ND4Params<P_, Q_> prm;
   prm.lidx = lidx + (size_t)e_off * op->PS;
   prm.qd = op->geom->qd + (size_t)e_off * 10 * op->geom->Q;
   prm.aq = op->aq ? op->aq + (size_t)e_off * op->aq_estride : nullptr;
@@ -920,28 +910,12 @@ int launch4(b2p_op *op, const int32_t *lidx, double alpha, const double *x, doub
   prm.y = y;
   prm.alpha = alpha;
   prm.ne = e_cnt;
-  prm.sp.n_owned = rg.n_owned < 0 ? op->lsize : rg.n_owned;
-  prm.sp.xg = rg.xg;
-  prm.sp.yg = rg.yg;
-  prm.wait_flags = rg.wait_flags;
-  prm.wait_expect = rg.wait_expect;
-  prm.wait_n = rg.wait_n;
-  prm.wait_from_elem = rg.wait_from_elem;
+  set_split_wait(prm, op, rg);
   prm.iso = op->iso ? 1 : 0;
-  const int n = P_ + 1;
-  for (int i = 0; i < Q_ * P_; i++) prm.Bo[i] = op->h_tab[i];
-  for (int i = 0; i < Q_ * n; i++) prm.Bc[i] = op->h_tab[Q_ * P_ + i];
-  for (int i = 0; i < Q_ * n; i++) prm.Gc[i] = op->h_tab[Q_ * P_ + Q_ * n + i];
+  copy_tables(op->h_tab.data(), P_, Q_, Q_, prm.Bo, prm.Bc, prm.Gc);
   const int nb = (e_cnt + L::NEW - 1) / L::NEW;
-  int grid = op->ctx->sm_count * MINB;
-  if (grid > (nb + NW - 1) / NW) grid = (nb + NW - 1) / NW;
-  record_launch(op->ctx, "nd_hex_apply4_kernel", false, false, op->ctx->sm_count * MINB, grid, NW, L::NEW, nb);
-  if (rg.pdl)
-    B2P_LAUNCH_PDL(kern, grid, NW * 32, shmem, s, prm);
-  else
-    B2P_LAUNCH(kern, grid, NW * 32, shmem, s, prm);
-  B2P_CUDA(op->ctx, cudaGetLastError());
-  return B2P_SUCCESS;
+  return launch_persistent(kern, prm, NW * 32, shmem, s, rg.pdl, op->ctx, "nd_hex_apply4_kernel", false, false, op->ctx->sm_count * MINB, NW,
+                           L::NEW, nb);
 }
 
 template <int P_, int Q_>
@@ -984,13 +958,8 @@ int launch4z(b2p_op *op, const int32_t *lidx, const double *zcoef, int has_imag,
     constexpr int NW = (WPS / MINB) < 1 ? 1 : WPS / MINB;
     const size_t shmem = (size_t)NW * L::WS;
     auto kern = nd_hex_apply4_kernel<P_, Q_, KIND, false, false, NW, MINB, true>;
-    static bool configured = false;
-    if (!configured)
-    {
-      B2P_CUDA(op->ctx, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)shmem));
-      configured = true;
-    }
     if (op->ne <= 0) return B2P_SUCCESS;
+    if (int rc = configure_kernel(op->ctx, kern, shmem)) return rc;
     ND4ParamsZ<P_, Q_> prm;
     prm.lidx = lidx;
     prm.qd = op->geom->qd;
@@ -1002,29 +971,16 @@ int launch4z(b2p_op *op, const int32_t *lidx, const double *zcoef, int has_imag,
     prm.y = yr;
     prm.alpha = alpha;
     prm.ne = op->ne;
-    prm.sp.n_owned = op->lsize;
-    prm.sp.xg = nullptr;
-    prm.sp.yg = nullptr;
-    prm.wait_flags = nullptr;
-    prm.wait_expect = nullptr;
-    prm.wait_n = 0;
-    prm.wait_from_elem = 0;
+    set_split_wait(prm, op, ApplyRange());
     prm.iso = 0;
     prm.xi = xi;
     prm.yi = yi;
     prm.zcoef = zcoef;
     prm.has_imag = has_imag;
-    const int n = P_ + 1;
-    for (int i = 0; i < Q_ * P_; i++) prm.Bo[i] = op->h_tab[i];
-    for (int i = 0; i < Q_ * n; i++) prm.Bc[i] = op->h_tab[Q_ * P_ + i];
-    for (int i = 0; i < Q_ * n; i++) prm.Gc[i] = op->h_tab[Q_ * P_ + Q_ * n + i];
+    copy_tables(op->h_tab.data(), P_, Q_, Q_, prm.Bo, prm.Bc, prm.Gc);
     const int nb = (op->ne + L::NEB - 1) / L::NEB;
-    int grid = op->ctx->sm_count * MINB;
-    if (grid > (nb + NW - 1) / NW) grid = (nb + NW - 1) / NW;
-    record_launch(op->ctx, "nd_hex_apply4_kernel", false, true, op->ctx->sm_count * MINB, grid, NW, L::NEB, nb);
-    B2P_LAUNCH(kern, grid, NW * 32, shmem, s, prm);
-    B2P_CUDA(op->ctx, cudaGetLastError());
-    return B2P_SUCCESS;
+    return launch_persistent(kern, prm, NW * 32, shmem, s, false, op->ctx, "nd_hex_apply4_kernel", false, true, op->ctx->sm_count * MINB, NW,
+                             L::NEB, nb);
   }
 }
 

@@ -627,27 +627,6 @@ __global__ void __launch_bounds__(NW * 32, MINB) nd_hex_apply5_kernel(const __gr
   }
 }
 
-// Mirror symmetry of the packed 1-D tables (Bo | Bc | Gc, each [q][len]) the kernel relies on.
-bool tables_symmetric(const double *tab, int p, int q)
-{
-  const int n = p + 1;
-  const double *Bo = tab, *Bc = tab + q * p, *Gc = Bc + q * n;
-  double scale = 0.0;
-  for (int i = 0; i < q * p + 2 * q * n; i++) scale = std::fmax(scale, std::fabs(tab[i]));
-  const double tol = 1e-13 * scale;
-  for (int c = 0; c < q; c++)
-  {
-    for (int i = 0; i < p; i++)
-      if (std::fabs(Bo[c * p + i] - Bo[(q - 1 - c) * p + (p - 1 - i)]) > tol) return false;
-    for (int i = 0; i < n; i++)
-    {
-      if (std::fabs(Bc[c * n + i] - Bc[(q - 1 - c) * n + (n - 1 - i)]) > tol) return false;
-      if (std::fabs(Gc[c * n + i] + Gc[(q - 1 - c) * n + (n - 1 - i)]) > tol) return false;
-    }
-  }
-  return true;
-}
-
 template <int P_, int KIND, bool ASM, int MINB_WANT>
 int launch5(b2p_op *op, const int32_t *lidx, double alpha, const double *x, double *y, const ApplyRange &rg, cudaStream_t s)
 {
@@ -657,18 +636,12 @@ int launch5(b2p_op *op, const int32_t *lidx, double alpha, const double *x, doub
   constexpr int FIT = (int)((228 * 1024) / (shmem + 1024));  // CTAs per SM that fit in shared memory
   constexpr int MINB = MINB_WANT < FIT ? MINB_WANT : FIT;
   static_assert(MINB >= 1, "shared memory per SM");
-  const bool split = rg.xg || rg.yg || (rg.n_owned >= 0 && rg.n_owned < op->lsize);
+  const bool split = range_split(op, rg);
   auto kern = split ? nd_hex_apply5_kernel<P_, KIND, ASM, true, NW, MINB> : nd_hex_apply5_kernel<P_, KIND, ASM, false, NW, MINB>;
-  static bool configured[2] = {false, false};
-  if (!configured[split])
-  {
-    B2P_CUDA(op->ctx, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)shmem));
-    B2P_CUDA(op->ctx, cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
-    configured[split] = true;
-  }
-  ND5Params<P_> prm;
-  const int e_off = rg.e_off, e_cnt = rg.e_cnt < 0 ? op->ne - rg.e_off : rg.e_cnt;
+  const int e_off = rg.e_off, e_cnt = range_count(op, rg);
   if (e_cnt <= 0) return B2P_SUCCESS;
+  if (int rc = configure_kernel(op->ctx, kern, shmem, cudaSharedmemCarveoutMaxShared)) return rc;
+  ND5Params<P_> prm;
   prm.lidx = lidx + (size_t)e_off * op->PS;
   prm.qd = op->geom->qd + (size_t)e_off * 10 * op->geom->Q;
   prm.aq = op->aq ? op->aq + (size_t)e_off * op->aq_estride : nullptr;
@@ -677,24 +650,11 @@ int launch5(b2p_op *op, const int32_t *lidx, double alpha, const double *x, doub
   prm.y = y;
   prm.alpha = alpha;
   prm.ne = e_cnt;
-  prm.sp.n_owned = rg.n_owned < 0 ? op->lsize : rg.n_owned;
-  prm.sp.xg = rg.xg;
-  prm.sp.yg = rg.yg;
-  prm.wait_flags = rg.wait_flags;
-  prm.wait_expect = rg.wait_expect;
-  prm.wait_n = rg.wait_n;
-  prm.wait_from_elem = rg.wait_from_elem;
+  set_split_wait(prm, op, rg);
   prm.iso = op->iso ? 1 : 0;
-  constexpr int n = P_ + 1, q = 4;
-  for (int i = 0; i < q * P_; i++) prm.Bo[i] = op->h_tab[i];
-  for (int i = 0; i < q * n; i++) prm.Bc[i] = op->h_tab[q * P_ + i];
-  for (int i = 0; i < q * n; i++) prm.Gc[i] = op->h_tab[q * P_ + q * n + i];
-  int grid = op->ctx->sm_count * MINB;
-  if (grid > (e_cnt + NW - 1) / NW) grid = (e_cnt + NW - 1) / NW;
-  record_launch(op->ctx, "nd_hex_apply5_kernel", false, false, op->ctx->sm_count * MINB, grid, NW, 1, e_cnt);
-  B2P_LAUNCH(kern, grid, NW * 32, shmem, s, prm);
-  B2P_CUDA(op->ctx, cudaGetLastError());
-  return B2P_SUCCESS;
+  copy_tables(op->h_tab.data(), P_, 4, 4, prm.Bo, prm.Bc, prm.Gc);
+  return launch_persistent(kern, prm, NW * 32, shmem, s, false, op->ctx, "nd_hex_apply5_kernel", false, false, op->ctx->sm_count * MINB, NW, 1,
+                           e_cnt);
 }
 
 template <int P_, int MINB>
@@ -722,9 +682,7 @@ int launch5_kind(b2p_op *op, const int32_t *lidx, double alpha, const double *x,
 // True when this operator can run on the one-element-per-warp kernel.
 bool nd_hex_apply5_eligible(b2p_op *op)
 {
-  if (op->q1d != 4 || op->p != 3) return false;
-  if (op->tab_sym < 0) op->tab_sym = tables_symmetric(op->h_tab.data(), op->p, op->q1d) ? 1 : 0;
-  return op->tab_sym == 1;
+  return op->q1d == 4 && op->p == 3 && nd_tables_symmetric(op, 1e-13);
 }
 
 int launch_nd_hex_apply5(b2p_op *op, const int32_t *lidx, double alpha, const double *x, double *y, const ApplyRange &rg, cudaStream_t s)

@@ -1001,7 +1001,7 @@ int launch6_cfg(b2p_op *op, const int32_t *lidx, double alpha, const double *x, 
 {
   using L = ND6Layout<P_, Q_, KIND, FWD, GSM, NODES>;
   const size_t shmem = (size_t)NW * L::WS;
-  const bool split = rg.xg || rg.yg || (rg.n_owned >= 0 && rg.n_owned < op->lsize);
+  const bool split = range_split(op, rg);
   auto kern = nd_hex_apply6_kernel<P_, Q_, KIND, false, NW, MINB, FWD, GSM, XLATE, GL1, NODES>;
   if constexpr (WITH_SPLIT)
   {
@@ -1012,19 +1012,12 @@ int launch6_cfg(b2p_op *op, const int32_t *lidx, double alpha, const double *x, 
     set_error(op->ctx, "nd_hex_apply6: this experimental configuration has no owned/ghost split variant");
     return B2P_ERR_UNSUPPORTED;
   }
-  static bool configured[2] = {false, false};
-  if (!configured[split ? 1 : 0])
-  {
-    B2P_CUDA(op->ctx, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)shmem));
-#ifndef B2P_EMU
-    if (GL1)  // leave the rest of the 256 KB array to L1: it is the staging buffer of the q-data
-      cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, (int)((MINB * (shmem + 1024) * 100 + 228 * 1024 - 1) / (228 * 1024)));
-#endif
-    configured[split ? 1 : 0] = true;
-  }
-  ND6Params<P_, Q_> prm;
-  const int e_off = rg.e_off, e_cnt = rg.e_cnt < 0 ? op->ne - rg.e_off : rg.e_cnt;
+  const int e_off = rg.e_off, e_cnt = range_count(op, rg);
   if (e_cnt <= 0) return B2P_SUCCESS;
+  // GL1: leave the rest of the 256 KB array to L1, the staging buffer of the q-data
+  const int carveout = GL1 ? (int)((MINB * (shmem + 1024) * 100 + 228 * 1024 - 1) / (228 * 1024)) : -1;
+  if (int rc = configure_kernel(op->ctx, kern, shmem, carveout)) return rc;
+  ND6Params<P_, Q_> prm;
   prm.lidx = lidx + (size_t)e_off * op->PS;
   prm.qd = op->geom->qd + (size_t)e_off * 10 * op->geom->Q;
   prm.xe = NODES ? op->geom->xe + (size_t)e_off * L::NE8 : nullptr;
@@ -1037,32 +1030,15 @@ int launch6_cfg(b2p_op *op, const int32_t *lidx, double alpha, const double *x, 
   prm.sink = op->ctx->d_sink;
   prm.alpha = alpha;
   prm.ne = e_cnt;
-  prm.sp.n_owned = rg.n_owned < 0 ? op->lsize : rg.n_owned;
-  prm.sp.xg = rg.xg;
-  prm.sp.yg = rg.yg;
-  prm.wait_flags = rg.wait_flags;
-  prm.wait_expect = rg.wait_expect;
-  prm.wait_n = rg.wait_n;
-  prm.wait_from_elem = rg.wait_from_elem;
+  set_split_wait(prm, op, rg);
   prm.iso = (op->iso && !L::BLOCK) ? 1 : 0;
-  const int n = P_ + 1;
-  constexpr int H = ND6Params<P_, Q_>::H;
-  for (int i = 0; i < H * P_; i++) prm.Bo[i] = op->h_tab[i];
-  for (int i = 0; i < H * n; i++) prm.Bc[i] = op->h_tab[Q_ * P_ + i];
-  for (int i = 0; i < H * n; i++) prm.Gc[i] = op->h_tab[Q_ * P_ + Q_ * n + i];
+  copy_tables(op->h_tab.data(), P_, Q_, ND6Params<P_, Q_>::H, prm.Bo, prm.Bc, prm.Gc);  // the first H rows: the rest mirror them
   for (int i = 0; i < 2 * Q_; i++) prm.nB[i] = NODES ? op->geom->h_nodeB[i] : 0.0;
   for (int i = 0; i < 2 * Q_; i++) prm.nG[i] = NODES ? op->geom->h_nodeG[i] : 0.0;
   for (int i = 0; i < Q_; i++) prm.qw[i] = NODES ? op->geom->h_qw[i] : 0.0;
   const int nb = (e_cnt + L::NEW - 1) / L::NEW;
-  int grid = op->ctx->sm_count * MINB;
-  if (grid > (nb + NW - 1) / NW) grid = (nb + NW - 1) / NW;
-  record_launch(op->ctx, "nd_hex_apply6_kernel", L::BLOCK, false, op->ctx->sm_count * MINB, grid, NW, L::NEW, nb, NODES);
-  if (rg.pdl)
-    B2P_LAUNCH_PDL(kern, grid, NW * 32, shmem, s, prm);
-  else
-    B2P_LAUNCH(kern, grid, NW * 32, shmem, s, prm);
-  B2P_CUDA(op->ctx, cudaGetLastError());
-  return B2P_SUCCESS;
+  return launch_persistent(kern, prm, NW * 32, shmem, s, rg.pdl, op->ctx, "nd_hex_apply6_kernel", L::BLOCK, false, op->ctx->sm_count * MINB, NW,
+                           L::NEW, nb, NODES);
 }
 
 // B2P_ND6_CFG = "<warps per CTA><CTAs per SM><f|y><g|l|c|n><e|x>" picks another launch shape / variant of the p = 3
@@ -1127,33 +1103,11 @@ int launch6(b2p_op *op, const int32_t *lidx, double alpha, const double *x, doub
 
 }  // namespace
 
-// Mirror symmetry of the 1-D tables to round-off (the half-table kernels substitute mirrored entries).
-bool nd_tables_symmetric(const double *tab, int p, int q, double rel_tol)
-{
-  const int n = p + 1;
-  const double *Bo = tab, *Bc = tab + q * p, *Gc = Bc + q * n;
-  double scale = 0.0;
-  for (int i = 0; i < q * p + 2 * q * n; i++) scale = std::fmax(scale, std::fabs(tab[i]));
-  const double tol = rel_tol * scale;  // the kernels substitute mirrored entries: they must agree to round-off
-  for (int c = 0; c < q; c++)
-  {
-    for (int i = 0; i < p; i++)
-      if (std::fabs(Bo[c * p + i] - Bo[(q - 1 - c) * p + (p - 1 - i)]) > tol) return false;
-    for (int i = 0; i < n; i++)
-    {
-      if (std::fabs(Bc[c * n + i] - Bc[(q - 1 - c) * n + (n - 1 - i)]) > tol) return false;
-      if (std::fabs(Gc[c * n + i] + Gc[(q - 1 - c) * n + (n - 1 - i)]) > tol) return false;
-    }
-  }
-  return true;
-}
-
 bool nd_hex_apply6_eligible(b2p_op *op)
 {
   if (!op || op->dense || op->assembled || op->kind == B2P_H1_DIFFUSION || !(op->ecoef || op->bcoef)) return false;
   if (!(op->q1d == op->p + 1 && op->p >= 2 && op->p <= 3)) return false;
-  if (op->tab_sym6 < 0) op->tab_sym6 = nd_tables_symmetric(op->h_tab.data(), op->p, op->q1d, 4e-16) ? 1 : 0;
-  return op->tab_sym6 == 1;
+  return nd_tables_symmetric(op, 4e-16);  // the kernel substitutes mirrored entries: they must agree to round-off
 }
 
 // Node geometry for the symmetric kinds at p = 3 only. The block form is already at 253-255 registers on the stored q-data and

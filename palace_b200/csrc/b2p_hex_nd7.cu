@@ -929,17 +929,12 @@ int launch7_cfg(b2p_op *op, const int32_t *lidx, double alpha, const double *x, 
   using L = ND7Layout<P_, KIND, NE>;
   constexpr int NT = 3 * WPC * 32;
   const size_t shmem = GSM ? L::SMEM_BYTES_GSM : L::SMEM_BYTES_LDG;
-  const bool split = rg.xg || rg.yg || (rg.n_owned >= 0 && rg.n_owned < op->lsize);
+  const bool split = range_split(op, rg);
   auto kern = split ? nd_hex_apply7_kernel<P_, KIND, true, NE, WPC, MINB, GSM, CBAR> : nd_hex_apply7_kernel<P_, KIND, false, NE, WPC, MINB, GSM, CBAR>;
-  static bool configured[2] = {false, false};
-  if (!configured[split ? 1 : 0])
-  {
-    B2P_CUDA(op->ctx, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)shmem));
-    configured[split ? 1 : 0] = true;
-  }
-  ND7Params<P_> prm;
-  const int e_off = rg.e_off, e_cnt = rg.e_cnt < 0 ? op->ne - rg.e_off : rg.e_cnt;
+  const int e_off = rg.e_off, e_cnt = range_count(op, rg);
   if (e_cnt <= 0) return B2P_SUCCESS;
+  if (int rc = configure_kernel(op->ctx, kern, shmem)) return rc;
+  ND7Params<P_> prm;
   prm.lidx = lidx + (size_t)e_off * op->PS;
   prm.qd = op->geom->qd + (size_t)e_off * 10 * op->geom->Q;
   if constexpr (L::BLOCK)
@@ -951,28 +946,12 @@ int launch7_cfg(b2p_op *op, const int32_t *lidx, double alpha, const double *x, 
   prm.sink = op->ctx->d_sink;
   prm.alpha = alpha;
   prm.ne = e_cnt;
-  prm.sp.n_owned = rg.n_owned < 0 ? op->lsize : rg.n_owned;
-  prm.sp.xg = rg.xg;
-  prm.sp.yg = rg.yg;
-  prm.wait_flags = rg.wait_flags;
-  prm.wait_expect = rg.wait_expect;
-  prm.wait_n = rg.wait_n;
-  prm.wait_from_elem = rg.wait_from_elem;
+  set_split_wait(prm, op, rg);
   prm.iso = (op->iso && !L::BLOCK) ? 1 : 0;
-  constexpr int q = P_ + 1, n = P_ + 1;
-  for (int i = 0; i < q * P_; i++) prm.Bo[i] = op->h_tab[i];
-  for (int i = 0; i < q * n; i++) prm.Bc[i] = op->h_tab[q * P_ + i];
-  for (int i = 0; i < q * n; i++) prm.Gc[i] = op->h_tab[q * P_ + q * n + i];
+  copy_tables(op->h_tab.data(), P_, P_ + 1, P_ + 1, prm.Bo, prm.Bc, prm.Gc);
   const int nb = (e_cnt + NE - 1) / NE;
-  int grid = op->ctx->sm_count * MINB;
-  if (grid > nb) grid = nb;
-  record_launch(op->ctx, "nd_hex_apply7_kernel", L::BLOCK, false, op->ctx->sm_count * MINB, grid, 1, NE, nb);
-  if (rg.pdl)
-    B2P_LAUNCH_PDL(kern, grid, NT, shmem, s, prm);
-  else
-    B2P_LAUNCH(kern, grid, NT, shmem, s, prm);
-  B2P_CUDA(op->ctx, cudaGetLastError());
-  return B2P_SUCCESS;
+  return launch_persistent(kern, prm, NT, shmem, s, rg.pdl, op->ctx, "nd_hex_apply7_kernel", L::BLOCK, false, op->ctx->sm_count * MINB, 1, NE,
+                           nb);
 }
 
 // Complex apply: one launch for both parts (see ND7ParamsZ); `op` supplies geometry, restriction and tables.
@@ -985,13 +964,8 @@ int launch7z(b2p_op *op, const int32_t *lidx, const double *coef, const double *
   constexpr int NT = 3 * S::WPC * 32;
   constexpr size_t shmem = L::SMEM_BYTES_GSM;
   auto kern = nd_hex_apply7_kernel<P_, KIND, false, S::NE, S::WPC, S::MINB_CPLX, true, S::CBAR, true>;
-  static bool configured = false;
-  if (!configured)
-  {
-    B2P_CUDA(op->ctx, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)shmem));
-    configured = true;
-  }
   if (op->ne <= 0) return B2P_SUCCESS;
+  if (int rc = configure_kernel(op->ctx, kern, shmem)) return rc;
   ND7ParamsZ<P_> prm;
   prm.lidx = lidx;
   prm.qd = op->geom->qd;
@@ -1006,25 +980,12 @@ int launch7z(b2p_op *op, const int32_t *lidx, const double *coef, const double *
   prm.sgn = sgn;
   prm.has_imag = has_imag;
   prm.ne = op->ne;
-  prm.sp.n_owned = op->lsize;
-  prm.sp.xg = nullptr;
-  prm.sp.yg = nullptr;
-  prm.wait_flags = nullptr;
-  prm.wait_expect = nullptr;
-  prm.wait_n = 0;
-  prm.wait_from_elem = 0;
+  set_split_wait(prm, op, ApplyRange());
   prm.iso = 0;
-  constexpr int q = P_ + 1, n = P_ + 1;
-  for (int i = 0; i < q * P_; i++) prm.Bo[i] = op->h_tab[i];
-  for (int i = 0; i < q * n; i++) prm.Bc[i] = op->h_tab[q * P_ + i];
-  for (int i = 0; i < q * n; i++) prm.Gc[i] = op->h_tab[q * P_ + q * n + i];
+  copy_tables(op->h_tab.data(), P_, P_ + 1, P_ + 1, prm.Bo, prm.Bc, prm.Gc);
   const int nb = (op->ne + S::NE - 1) / S::NE;
-  int grid = op->ctx->sm_count * S::MINB_CPLX;
-  if (grid > nb) grid = nb;
-  record_launch(op->ctx, "nd_hex_apply7_kernel", L::BLOCK, true, op->ctx->sm_count * S::MINB_CPLX, grid, 1, S::NE, nb);
-  B2P_LAUNCH(kern, grid, NT, shmem, s, prm);
-  B2P_CUDA(op->ctx, cudaGetLastError());
-  return B2P_SUCCESS;
+  return launch_persistent(kern, prm, NT, shmem, s, false, op->ctx, "nd_hex_apply7_kernel", L::BLOCK, true, op->ctx->sm_count * S::MINB_CPLX, 1,
+                           S::NE, nb);
 }
 
 // B2P_ND7_CFG = "<elements per batch><warps per component><CTAs per SM><d | g | c>" picks another launch shape of the
@@ -1087,8 +1048,7 @@ bool nd_hex_apply7_eligible(b2p_op *op)
   // The kernel reads mirrored table entries through one stored value. Tables evaluated in floating point (MFEM's, or
   // tests/hexspace.py) mirror to a few ulp of the LARGEST entry (measured 6e-16 ... 9e-16 at p = 4, 5): the substitution
   // changes the operator by less than the tables' own rounding.
-  if (op->tab_sym7 < 0) op->tab_sym7 = nd_tables_symmetric(op->h_tab.data(), op->p, op->q1d, 8e-15) ? 1 : 0;
-  return op->tab_sym7 == 1;
+  return nd_tables_symmetric(op, 8e-15);
 }
 
 int launch_nd_hex_apply7(b2p_op *op, const int32_t *lidx, double alpha, const double *x, double *y, const ApplyRange &rg, cudaStream_t s,

@@ -384,12 +384,7 @@ int launch_rt_pq(b2p_op *op, const int32_t *lidx, double alpha, const double *x,
   constexpr int NT = 256;
   const size_t shmem = (size_t)(Q_ * P_ + Q_ * (P_ + 1) + NEB * L::PER_ELEM) * sizeof(double);
   auto kern = rt_hex_apply_kernel<P_, Q_, NEB, NT>;
-  static bool configured = false;
-  if (!configured)
-  {
-    B2P_CUDA(op->ctx, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)shmem));
-    configured = true;
-  }
+  if (int rc = configure_kernel(op->ctx, kern, shmem)) return rc;
   B2P_LAUNCH(kern, (e_cnt + NEB - 1) / NEB, NT, shmem, s, make_rt_params(op, lidx, alpha, x, y, e_off, e_cnt));
   B2P_CUDA(op->ctx, cudaGetLastError());
   return B2P_SUCCESS;
@@ -402,12 +397,7 @@ int launch_rt7(b2p_op *op, const int32_t *lidx, double alpha, const double *x, d
   using L = RT7Layout<P_, S::NE>;
   constexpr int NT = 3 * S::WPC * 32;
   auto kern = rt_hex_apply7_kernel<P_, S::NE, S::WPC, S::MINB>;
-  static bool configured = false;
-  if (!configured)
-  {
-    B2P_CUDA(op->ctx, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)L::SMEM_BYTES));
-    configured = true;
-  }
+  if (int rc = configure_kernel(op->ctx, kern, L::SMEM_BYTES)) return rc;
   RT7Params<P_> prm;
   prm.lidx = lidx + (size_t)e_off * op->PS;
   prm.qd = op->geom->qd + (size_t)e_off * L::GE;
@@ -418,9 +408,7 @@ int launch_rt7(b2p_op *op, const int32_t *lidx, double alpha, const double *x, d
   prm.alpha = alpha;
   prm.ne = e_cnt;
   prm.PS = op->PS;
-  constexpr int q = P_ + 1, n = P_ + 1;
-  for (int i = 0; i < q * P_; i++) prm.Bo[i] = op->h_tab[i];
-  for (int i = 0; i < q * n; i++) prm.Bc[i] = op->h_tab[q * P_ + i];
+  copy_tables(op->h_tab.data(), P_, P_ + 1, P_ + 1, prm.Bo, prm.Bc, nullptr);
   B2P_LAUNCH(kern, (e_cnt + S::NE - 1) / S::NE, NT, L::SMEM_BYTES, s, prm);
   B2P_CUDA(op->ctx, cudaGetLastError());
   return B2P_SUCCESS;
@@ -433,17 +421,16 @@ bool rt_hex_apply7_eligible(b2p_op *op)
   // the same test as nd_hex_apply7_eligible: q1d = p + 1, p = 2 ... 6, tables mirror-symmetric within 8e-15 of the largest entry
   if (!op || op->kind != B2P_RT_MASS || op->dense || !op->ecoef) return false;
   if (!(op->q1d == op->p + 1 && op->p >= 2 && op->p <= 6)) return false;
-  if (op->tab_sym7 < 0) op->tab_sym7 = nd_tables_symmetric(op->h_tab.data(), op->p, op->q1d, 8e-15) ? 1 : 0;
-  return op->tab_sym7 == 1;
+  return nd_tables_symmetric(op, 8e-15);
 }
 
 int launch_rt_hex_apply(b2p_op *op, const int32_t *lidx, double alpha, const double *x, double *y, const ApplyRange &rg, cudaStream_t s,
-                        bool simple)
+                        bool rt7)
 {
-  const int e_off = rg.e_off, e_cnt = rg.e_cnt < 0 ? op->ne - rg.e_off : rg.e_cnt;
+  const int e_off = rg.e_off, e_cnt = range_count(op, rg);
   if (e_cnt <= 0) return B2P_SUCCESS;
   static const bool trace = std::getenv("B2P_TRACE_KERNEL") != nullptr;
-  if (!simple && rt_hex_apply7_eligible(op))
+  if (rt7)
   {
     if (trace) fprintf(stderr, "[b2p] rt_hex_apply7 p=%d q1d=%d ne=%d\n", op->p, op->q1d, e_cnt);
 #define B2P_CASE(PP) \

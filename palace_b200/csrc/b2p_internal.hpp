@@ -144,9 +144,9 @@ struct b2p_op
   int32_t *emat = nullptr;     // [ne][2] indices into mat (value part, derivative part)
   int n_mat = 0;
   bool iso = false;            // every material matrix is c * I
-  int tab_sym = -1;            // 1-D tables mirror-symmetric (nd_hex_apply5_kernel): -1 unknown, 0 no, 1 yes
-  int tab_sym6 = -1;           // same to round-off (nd_hex_apply6_kernel stores half the rows)
-  int tab_sym7 = -1;           // same within 8e-15 of the largest entry (nd_hex_apply7_kernel, p = 4, 5, 6)
+  // mirror symmetry of the 1-D tables (nd_tables_symmetric), computed on first use: the largest deviation from it and the
+  // largest |entry|; tab_dev < 0: not computed yet
+  double tab_dev = -1.0, tab_scale = 0.0;
   double *ecoef = nullptr;     // [ne][18] per-element coefficient matrices (TMA-friendly copy of mat[emat])
   // assembled q-data (optional): aq[ne][ncomp][Q], symmetric 6 per part
   double *aq = nullptr;
@@ -227,6 +227,87 @@ inline void record_launch(b2p_ctx *c, const char *kernel, bool block, bool cplx,
   r.batches = batches;
   r.seq++;
 }
+// Elements [rg.e_off, rg.e_off + range_count) of an apply range; <= 0: nothing to launch.
+inline int range_count(const b2p_op *op, const ApplyRange &rg) { return rg.e_cnt < 0 ? op->ne - rg.e_off : rg.e_cnt; }
+// Does the L-vector come in two pieces (owned part in x / y, ghosts in xg / yg)?
+inline bool range_split(const b2p_op *op, const ApplyRange &rg) { return rg.xg || rg.yg || (rg.n_owned >= 0 && rg.n_owned < op->lsize); }
+// The owned/ghost split of an apply range on a kernel's params struct (ApplyRange(): one piece).
+template <typename Prm>
+void set_split(Prm &prm, const b2p_op *op, const ApplyRange &rg)
+{
+  prm.sp.n_owned = rg.n_owned < 0 ? op->lsize : rg.n_owned;
+  prm.sp.xg = rg.xg;
+  prm.sp.yg = rg.yg;
+}
+// The split and the peer-memory halo wait (ApplyRange(): one piece, no wait).
+template <typename Prm>
+void set_split_wait(Prm &prm, const b2p_op *op, const ApplyRange &rg)
+{
+  set_split(prm, op, rg);
+  prm.wait_flags = rg.wait_flags;
+  prm.wait_expect = rg.wait_expect;
+  prm.wait_n = rg.wait_n;
+  prm.wait_from_elem = rg.wait_from_elem;
+}
+// The first `rows` rows of the packed 1-D tables Bo[q][p] | Bc[q][p+1] | Gc[q][p+1] into a kernel's parameter block; a null
+// destination skips that table.
+inline void copy_tables(const double *h_tab, int p, int q, int rows, double *Bo, double *Bc, double *Gc)
+{
+  const int n = p + 1;
+  for (int i = 0; Bo && i < rows * p; i++) Bo[i] = h_tab[i];
+  for (int i = 0; Bc && i < rows * n; i++) Bc[i] = h_tab[q * p + i];
+  for (int i = 0; Gc && i < rows * n; i++) Gc[i] = h_tab[q * p + q * n + i];
+}
+// Allow `kern` `shmem` bytes of dynamic shared memory and, with carveout >= 0, set its preferred shared-memory carveout (percent
+// or a cudaSharedmemCarveout value). The attributes belong to the device current at the call, so this runs once per (kernel, device).
+int configure_kernel_once(b2p_ctx *ctx, const void *kern, size_t shmem, int carveout = -1);
+template <typename K>
+int configure_kernel(b2p_ctx *ctx, K *kern, size_t shmem, int carveout = -1)
+{
+  return configure_kernel_once(ctx, (const void *)kern, shmem, carveout);
+}
+// Launch a persistent element kernel: max_grid CTAs clamped to the CTAs the batches fill (`workers` per CTA each walk batch,
+// batch + W, ...), the launch record (record_launch's fields), programmatic stream serialisation only with `pdl` (kernels that
+// call griddep_wait()).
+template <typename K, typename Prm>
+int launch_persistent(K *kern, const Prm &prm, int threads, size_t shmem, cudaStream_t s, bool pdl, b2p_ctx *c, const char *kernel,
+                      bool block, bool cplx, int max_grid, int workers, int elems_per_batch, int64_t batches, bool nodes = false)
+{
+  int grid = max_grid;
+  if (grid > (batches + workers - 1) / workers) grid = (int)((batches + workers - 1) / workers);
+  record_launch(c, kernel, block, cplx, max_grid, grid, workers, elems_per_batch, batches, nodes);
+  if (pdl)
+    B2P_LAUNCH_PDL(kern, grid, threads, shmem, s, prm);
+  else
+    B2P_LAUNCH(kern, grid, threads, shmem, s, prm);
+  B2P_CUDA(c, cudaGetLastError());
+  return B2P_SUCCESS;
+}
+// The element kernel of an apply (choose_hex_kernel, b2p_core.cu).
+enum class HexKernel
+{
+  DENSE,
+  ND_SIMPLE,
+  ND4,
+  ND5,
+  ND6,
+  ND7,
+  H1_SIMPLE,
+  H1V3,
+  RT_SIMPLE,
+  RT7
+};
+HexKernel choose_hex_kernel(b2p_op *op, int flags);
+// The one-pass kernel of a complex sum of n_terms operators like `op` (b2p_complex.cu plans the sum).
+enum class HexComplexKernel
+{
+  NONE,
+  ND4Z,
+  ND7Z
+};
+HexComplexKernel choose_hex_complex_kernel(b2p_op *op, int n_terms);
+// Can b2p_op_apply_add_pair run the two vectors through one nd_hex_apply4_kernel<CPLX> launch?
+bool hex_pair_apply_eligible(b2p_op *op);
 // Kernel launchers (defined in the .cu files).
 int launch_nd_hex_apply(b2p_op *op, const int32_t *lidx, double alpha, const double *x, double *y, const ApplyRange &rg, cudaStream_t s,
                         bool transpose = false);
@@ -236,12 +317,14 @@ bool nd_hex_apply5_eligible(b2p_op *op);
 int launch_nd_hex_apply6(b2p_op *op, const int32_t *lidx, double alpha, const double *x, double *y, const ApplyRange &rg, cudaStream_t s,
                          bool transpose = false);
 bool nd_hex_apply6_eligible(b2p_op *op);
-// Does nd_hex_apply6_kernel, when apply_range sends op to it, evaluate the geometry from the vertices of a trilinear mesh (the
-// symmetric kinds at p = 3) instead of reading the stored q-data?
+// Does nd_hex_apply6_kernel, when choose_hex_kernel sends op to it, evaluate the geometry from the vertices of a trilinear mesh
+// (the symmetric kinds at p = 3) instead of reading the stored q-data?
 bool nd_hex_apply6_reads_nodes(const b2p_op *op);
-// Does apply_range send op, with these apply flags, to nd_hex_apply6_kernel?
-bool routes_to_nd6(b2p_op *op, int flags);
+// Are the packed 1-D tables Bo | Bc | Gc mirror-symmetric (Bo, Bc even, Gc odd about the centre) to within rel_tol times their
+// largest entry? The kernels that store half the rows or read mirrored entries through one value need it. The second form
+// reads op's tables through the deviation cached on op.
 bool nd_tables_symmetric(const double *tab, int p, int q, double rel_tol);
+bool nd_tables_symmetric(b2p_op *op, double rel_tol);
 int launch_nd_hex_apply7(b2p_op *op, const int32_t *lidx, double alpha, const double *x, double *y, const ApplyRange &rg, cudaStream_t s,
                          bool transpose = false);
 bool nd_hex_apply7_eligible(b2p_op *op);
@@ -259,11 +342,10 @@ bool op_essential_matches(const b2p_op *op, const int32_t *ess_ldofs, int64_t n)
 int apply_range(b2p_op *op, const int32_t *lidx, double alpha, const double *x, double *y, const ApplyRange &rg, int flags,
                 cudaStream_t s);
 int launch_nd_hex_diag(b2p_op *op, double *diag, cudaStream_t s);
-// Raviart-Thomas mass (b2p_hex_rt.cu): the production kernel where rt_hex_apply7_eligible holds and `simple` is not set, the
-// cross-check kernel otherwise
+// Raviart-Thomas mass (b2p_hex_rt.cu): rt_hex_apply7_kernel with `rt7`, the cross-check kernel otherwise
 bool rt_hex_apply7_eligible(b2p_op *op);
 int launch_rt_hex_apply(b2p_op *op, const int32_t *lidx, double alpha, const double *x, double *y, const ApplyRange &rg, cudaStream_t s,
-                        bool simple);
+                        bool rt7);
 int launch_rt_hex_diag(b2p_op *op, double *diag, cudaStream_t s);
 // Signed lexicographic restriction [ne][*PS] of the b2p_op_desc fields idx / orient / dof_map for P dofs per element (the one
 // restriction builder: b2p_op_create, b2p_op_coarsen and b2p_flux_estimator_create_hex); rows padded to *PS = P rounded up to 4

@@ -36,9 +36,9 @@ def test_product_library_has_no_emulation_code():
 @pytest.mark.parametrize("order", ["fwd", "rev"])
 def test_element_kernels_under_emulation(order):
     """Sum-factorised ND / H1 hex kernels (production, simple and half-warp variants), the dense DMMA operator,
-    the tetrahedron path, the fused complex kernel: every parity test of these files must also hold on the emulated SIMT machine, for two
+    the tetrahedron path, the fused complex kernel, the kernel each hex apply is routed to: every parity test of these files must also hold on the emulated SIMT machine, for two
     different lane execution orders (a missing warp barrier shows up as stale data in at least one of them)."""
-    n = _run(["tests/test_apply_gpu.py", "tests/test_dense_gpu.py", "tests/test_tet_gpu.py", "tests/test_zfused_gpu.py", "tests/test_zassemble_gpu.py", "tests/test_zbdr_gpu.py", "tests/test_zsolver_variants_gpu.py", "tests/test_zsum_gpu.py"], order)
+    n = _run(["tests/test_apply_gpu.py", "tests/test_dense_gpu.py", "tests/test_tet_gpu.py", "tests/test_zfused_gpu.py", "tests/test_zassemble_gpu.py", "tests/test_zbdr_gpu.py", "tests/test_zsolver_variants_gpu.py", "tests/test_zsum_gpu.py", "tests/test_zzhex_routes_gpu.py"], order)
     assert n >= 120
 
 
