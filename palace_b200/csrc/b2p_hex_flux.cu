@@ -1,14 +1,19 @@
-// Sum-factorised flux operator and element error integrals of the flux error estimators on hexahedra
-// (b2p_flux_estimator_create_hex): the same linear maps as mixed_mass_kernel / flux_error_kernel of b2p_flux.cu, with the 1-D
-// tables of the Nedelec space ND_p and the Raviart-Thomas space RT_{p-1} instead of dense [3][Q][P] tables.
+// Sum-factorised H(div) work on hexahedra: the Raviart-Thomas mass operator (kind B2P_RT_MASS), and the flux operator and element
+// error integrals of the flux error estimators (b2p_flux_estimator_create_hex). The RT mass and Flux are one mixed mass over a trial
+// space and a test space, with the 1-D tables of the Nedelec space ND_p and the Raviart-Thomas space RT_{p-1}:
 //
-//   mixed mass        y_test += sum_e E_test^T B_test^T D B_trial E_trial x_trial,   D = w detJ P_test^T C P_trial
-//   error integral    est[e] += sum_q w detJ | C2 P2 u2 - C1 P1 u1 |^2              (u_i = B_i E_i x_i)
+//   mixed mass        y_test += alpha sum_e E_test^T B_test^T D B_trial E_trial x_trial,   D = w detJ P_test^T C P_trial
+//   error integral    est[e] += sum_q w detJ | C2 P2 u2 - C1 P1 u1 |^2                     (u_i = B_i E_i x_i)
 //
 // P_HCURL = A (the stored adj(J)^T / detJ), P_HDIV = Jd = cofactor(A); C is a general (possibly non-symmetric) 3x3 per element.
+//   RT mass       (RT, RT): VectorFEMassIntegrator on an RT space, D = (w / detJ) J^T C J = w detJ Jd^T C Jd, the quadrature
+//                 function f_apply_hdiv_33 (fem/integ/vecfemass.cpp:80-86, qfunctions/33/hdiv_33_qf.h:10-30); the operator inside
+//                 the FluxProjector's PCG of GradFluxErrorEstimator (linalg/errorestimator.cpp:272-398). C: the first 9 of b2p_op::ecoef.
+//   Flux          (ND, RT) or (RT, ND), and the error integrals: the same linear maps as mixed_mass_kernel / flux_error_kernel of
+//                 b2p_flux.cu, with 1-D tables instead of dense [3][Q][P] tables.
 // Both spaces share p (the ND-equivalent order), q1d and the tables Bo[q1d][p], Bc[q1d][p+1]. Lexicographic element layouts:
 //   ND component c: open (p) along axis c, closed (p + 1) along the other two, offset c p (p+1)^2   (b2p_hex_nd.cu)
-//   RT component c: closed along axis c, open along the other two,             offset c (p+1) p^2   (b2p_hex_rt.cu)
+//   RT component c: closed along axis c, open along the other two,             offset c (p+1) p^2   (hexspace._rt_lex_layout)
 //
 // Kernels:
 //   flux_hex_mixed7_kernel / flux_hex_error7_kernel   production, p = 2 ... 6 at q1d = p + 1 with mirror-symmetric tables: one CTA
@@ -17,8 +22,10 @@
 //        RED.F64 (masked entries add 0.0 to a sink slot), the error integral runs the forward phases of both spaces over the same
 //        staged q-data;
 //   flux_hex_mixed_kernel / flux_hex_error_kernel     cross-check, every p <= 6 and p < q1d <= 7 (shared-memory contract<>), and
-//        the route wherever the production kernels are not eligible.
-// Every launch stores its kernel name in the context's launch record (b2p_ctx_last_launch): one batch per CTA, grid = batches.
+//        the route wherever the production kernels are not eligible (for the RT mass also under B2P_APPLY_SIMPLE_KERNEL);
+//   rt_hex_diag_kernel                                the diagonal of the RT mass, one thread per (element, dof).
+// Flux and error-integral launches store their kernel name in the context's launch record (b2p_ctx_last_launch): one batch per
+// CTA, grid = batches. RT mass launches leave the record alone.
 // The error integrals reduce each element's points in a fixed order (one warp per element: strided lane sums, then a butterfly),
 // so two calls give bit-identical estimates whatever the schedule.
 #include <cstdlib>
@@ -36,6 +43,8 @@ namespace
 
 constexpr int SP_ND = 0, SP_RT = 1;
 
+constexpr int imax(int a, int b) { return a > b ? a : b; }
+
 // extents of component C of space S along the three axes: ND open (p) along axis C and closed (p + 1) along the others, RT the
 // other way round
 template <int P_, int S, int C>
@@ -47,10 +56,16 @@ struct HexComp
   static constexpr int D3 = d0 * d1 * d2;
   static constexpr int off = C * D3;
 };
+// element dofs of space S, and the largest line counts over its components after the first contraction (d1 d2) and the second (d2)
 template <int P_, int S>
 struct HexSpace
 {
-  static constexpr int P = S == SP_ND ? 3 * P_ * (P_ + 1) * (P_ + 1) : 3 * (P_ + 1) * P_ * P_;
+  using K0 = HexComp<P_, S, 0>;
+  using K1 = HexComp<P_, S, 1>;
+  using K2 = HexComp<P_, S, 2>;
+  static constexpr int P = 3 * K0::D3;
+  static constexpr int D12 = imax(imax(K0::d1 * K0::d2, K1::d1 * K1::d2), K2::d1 * K2::d2);
+  static constexpr int D2 = imax(imax(K0::d2, K1::d2), K2::d2);
 };
 
 // physical value of a reference-space vector: H(curl) A u^, H(div) Jd u^
@@ -67,12 +82,12 @@ __device__ __forceinline__ void piola(const double A[9], double M[9])
 }
 
 // v = w detJ P_test^T C P_trial u
-template <int ST>
+template <int ST, int SS>
 __device__ __forceinline__ void mixed_point(const double A[9], const double C[9], double wdetj, const double u[3], double v[3])
 {
   double Mt[9], Ms[9], t[3], z[3];
   piola<ST>(A, Mt);
-  piola<1 - ST>(A, Ms);
+  piola<SS>(A, Ms);
   Ax33(Mt, u, t);
   Ax33(C, t, z);
   Atx33(Ms, z, wdetj, v);
@@ -107,14 +122,16 @@ __device__ __forceinline__ double warp_fixed_sum(const double *r, int cnt, int l
 
 // ---- cross-check kernels ------------------------------------------------------------------------------------------------
 
-template <int P_, int Q_, int NV>
+// SA, SB: the two spaces of the kernel; NV = 1: their element dofs one at a time (mixed mass), NV = 2: both (error integral)
+template <int P_, int Q_, int SA, int SB, int NV>
 struct HFLayout
 {
+  using Sa = HexSpace<P_, SA>;
+  using Sb = HexSpace<P_, SB>;
   static constexpr int p = P_, q = Q_, n = P_ + 1, Q = q * q * q;
-  static constexpr int PN = HexSpace<P_, SP_ND>::P, PR = HexSpace<P_, SP_RT>::P;
-  static constexpr int UE = NV == 1 ? PN : PN + PR;  // element dofs: one space at a time (mixed mass) or both (error integral)
-  static constexpr int N1 = q * n * n;                // after the first contraction (largest over the components of both spaces)
-  static constexpr int N2 = q * q * n;                // after the second
+  static constexpr int UE = NV == 1 ? imax(Sa::P, Sb::P) : Sa::P + Sb::P;  // element dofs
+  static constexpr int N1 = q * imax(Sa::D12, Sb::D12);                     // after the first contraction
+  static constexpr int N2 = q * q * imax(Sa::D2, Sb::D2);                   // after the second
   // per-element shared doubles: U | T1 | T2 | uq[NV][3Q]
   static constexpr int PER_ELEM = UE + N1 + N2 + NV * 3 * Q;
 };
@@ -129,16 +146,16 @@ struct HFParams
   int CE;
   const double *x_a, *x_b;
   double *y;            // the test space's L-vector (mixed mass) or the estimates [ne] (error integral)
+  double alpha;         // scale of the mixed mass
   int ne;
 };
 
 // element dofs U_C of space S (d0, d1, d2) -> values at the points (q, q, q)
-template <int P_, int Q_, int NV, int S, int C, int NEB, int NT>
+template <typename L, int S, int C, int NEB, int NT>
 __device__ __forceinline__ void hf_forward(const double *U, double *T1, double *T2, double *uq, const double *sBo, const double *sBc)
 {
-  using L = HFLayout<P_, Q_, NV>;
-  using K = HexComp<P_, S, C>;
-  constexpr int q = Q_, ES = L::PER_ELEM, d0 = K::d0, d1 = K::d1, d2 = K::d2;
+  using K = HexComp<L::p, S, C>;
+  constexpr int q = L::q, ES = L::PER_ELEM, d0 = K::d0, d1 = K::d1, d2 = K::d2;
   contract<0, d0, d1, d2, d0, q, false, NEB, NT>(U + K::off, ES, T1, ES, K::c0 ? sBc : sBo, d0, 1, 1.0);
   __syncthreads();
   contract<1, q, d1, d2, d1, q, false, NEB, NT>(T1, ES, T2, ES, K::c1 ? sBc : sBo, d1, 1, 1.0);
@@ -148,12 +165,11 @@ __device__ __forceinline__ void hf_forward(const double *U, double *T1, double *
 }
 
 // point values (q, q, q) -> element dofs U_C of space S (overwritten)
-template <int P_, int Q_, int NV, int S, int C, int NEB, int NT>
+template <typename L, int S, int C, int NEB, int NT>
 __device__ __forceinline__ void hf_transpose(double *U, double *T1, double *T2, const double *uq, const double *sBo, const double *sBc)
 {
-  using L = HFLayout<P_, Q_, NV>;
-  using K = HexComp<P_, S, C>;
-  constexpr int q = Q_, ES = L::PER_ELEM, d0 = K::d0, d1 = K::d1, d2 = K::d2;
+  using K = HexComp<L::p, S, C>;
+  constexpr int q = L::q, ES = L::PER_ELEM, d0 = K::d0, d1 = K::d1, d2 = K::d2;
   contract<2, q, q, q, q, d2, false, NEB, NT>(uq + C * L::Q, ES, T2, ES, K::c2 ? sBc : sBo, 1, d2, 1.0);
   __syncthreads();
   contract<1, q, q, d2, q, d1, false, NEB, NT>(T2, ES, T1, ES, K::c1 ? sBc : sBo, 1, d1, 1.0);
@@ -162,11 +178,10 @@ __device__ __forceinline__ void hf_transpose(double *U, double *T1, double *T2, 
   __syncthreads();
 }
 
-template <int P_, int Q_, int NV, int S, int NEB, int NT>
+template <typename L, int S, int NEB, int NT>
 __device__ __forceinline__ void hf_gather(const int32_t *lidx, int PS, const double *x, double *U, int e0, int ne)
 {
-  using L = HFLayout<P_, Q_, NV>;
-  constexpr int P = HexSpace<P_, S>::P;
+  constexpr int P = HexSpace<L::p, S>::P;
   for (int w = threadIdx.x; w < NEB * P; w += NT)
   {
     const int e = w / P, l = w % P;
@@ -174,22 +189,22 @@ __device__ __forceinline__ void hf_gather(const int32_t *lidx, int PS, const dou
   }
 }
 
-// ST: the trial space; the test space is the other one
-template <int P_, int Q_, int ST, int NEB, int NT>
+// ST: the trial space, SS: the test space
+template <int P_, int Q_, int ST, int SS, int NEB, int NT>
 __global__ void __launch_bounds__(NT) flux_hex_mixed_kernel(HFParams prm)
 {
-  using L = HFLayout<P_, Q_, 1>;
-  constexpr int p = L::p, q = L::q, n = L::n, Q = L::Q, ES = L::PER_ELEM, SS = 1 - ST, PT = HexSpace<P_, SS>::P;
+  using L = HFLayout<P_, Q_, ST, SS, 1>;
+  constexpr int p = L::p, q = L::q, n = L::n, Q = L::Q, ES = L::PER_ELEM, PT = HexSpace<P_, SS>::P;
   B2P_DYN_SMEM(double, smem);
   double *sBo = smem, *sBc = sBo + q * p, *work = sBc + q * n;
   double *U = work, *T1 = U + L::UE, *T2 = T1 + L::N1, *uq = T2 + L::N2;
   for (int i = threadIdx.x; i < q * p + q * n; i += NT) sBo[i] = prm.tab[i];
   const int e0 = blockIdx.x * NEB;
-  hf_gather<P_, Q_, 1, ST, NEB, NT>(prm.lidx_a, prm.PS_a, prm.x_a, U, e0, prm.ne);
+  hf_gather<L, ST, NEB, NT>(prm.lidx_a, prm.PS_a, prm.x_a, U, e0, prm.ne);
   __syncthreads();
-  hf_forward<P_, Q_, 1, ST, 0, NEB, NT>(U, T1, T2, uq, sBo, sBc);
-  hf_forward<P_, Q_, 1, ST, 1, NEB, NT>(U, T1, T2, uq, sBo, sBc);
-  hf_forward<P_, Q_, 1, ST, 2, NEB, NT>(U, T1, T2, uq, sBo, sBc);
+  hf_forward<L, ST, 0, NEB, NT>(U, T1, T2, uq, sBo, sBc);
+  hf_forward<L, ST, 1, NEB, NT>(U, T1, T2, uq, sBo, sBc);
+  hf_forward<L, ST, 2, NEB, NT>(U, T1, T2, uq, sBo, sBc);
   for (int w = threadIdx.x; w < NEB * Q; w += NT)
   {
     const int e = w / Q, iq = w % Q;
@@ -206,20 +221,20 @@ __global__ void __launch_bounds__(NT) flux_hex_mixed_kernel(HFParams prm)
     double *u = uq + e * ES;
     const double uu[3] = {u[iq], u[Q + iq], u[2 * Q + iq]};
     double v[3];
-    mixed_point<ST>(A, C, g[0], uu, v);
+    mixed_point<ST, SS>(A, C, g[0], uu, v);
     u[iq] = v[0];
     u[Q + iq] = v[1];
     u[2 * Q + iq] = v[2];
   }
   __syncthreads();
-  hf_transpose<P_, Q_, 1, SS, 0, NEB, NT>(U, T1, T2, uq, sBo, sBc);
-  hf_transpose<P_, Q_, 1, SS, 1, NEB, NT>(U, T1, T2, uq, sBo, sBc);
-  hf_transpose<P_, Q_, 1, SS, 2, NEB, NT>(U, T1, T2, uq, sBo, sBc);
+  hf_transpose<L, SS, 0, NEB, NT>(U, T1, T2, uq, sBo, sBc);
+  hf_transpose<L, SS, 1, NEB, NT>(U, T1, T2, uq, sBo, sBc);
+  hf_transpose<L, SS, 2, NEB, NT>(U, T1, T2, uq, sBo, sBc);
   for (int w = threadIdx.x; w < NEB * PT; w += NT)
   {
     const int e = w / PT, l = w % PT;
     if (e0 + e >= prm.ne) continue;
-    scatter1(prm.y, prm.lidx_b[(size_t)(e0 + e) * prm.PS_b + l], U[e * ES + l]);
+    scatter1(prm.y, prm.lidx_b[(size_t)(e0 + e) * prm.PS_b + l], prm.alpha * U[e * ES + l]);
   }
 }
 
@@ -227,22 +242,23 @@ __global__ void __launch_bounds__(NT) flux_hex_mixed_kernel(HFParams prm)
 template <int P_, int Q_, int S1, int NEB, int NT>
 __global__ void __launch_bounds__(NT) flux_hex_error_kernel(HFParams prm)
 {
-  using L = HFLayout<P_, Q_, 2>;
-  constexpr int p = L::p, q = L::q, n = L::n, Q = L::Q, ES = L::PER_ELEM, S2 = 1 - S1, P1 = HexSpace<P_, S1>::P;
+  constexpr int S2 = 1 - S1, P1 = HexSpace<P_, S1>::P;
+  using L = HFLayout<P_, Q_, S1, S2, 2>;
+  constexpr int p = L::p, q = L::q, n = L::n, Q = L::Q, ES = L::PER_ELEM;
   B2P_DYN_SMEM(double, smem);
   double *sBo = smem, *sBc = sBo + q * p, *work = sBc + q * n;
   double *U1 = work, *U2 = U1 + P1, *T1 = U1 + L::UE, *T2 = T1 + L::N1, *uq1 = T2 + L::N2, *uq2 = uq1 + 3 * Q;
   for (int i = threadIdx.x; i < q * p + q * n; i += NT) sBo[i] = prm.tab[i];
   const int e0 = blockIdx.x * NEB;
-  hf_gather<P_, Q_, 2, S1, NEB, NT>(prm.lidx_a, prm.PS_a, prm.x_a, U1, e0, prm.ne);
-  hf_gather<P_, Q_, 2, S2, NEB, NT>(prm.lidx_b, prm.PS_b, prm.x_b, U2, e0, prm.ne);
+  hf_gather<L, S1, NEB, NT>(prm.lidx_a, prm.PS_a, prm.x_a, U1, e0, prm.ne);
+  hf_gather<L, S2, NEB, NT>(prm.lidx_b, prm.PS_b, prm.x_b, U2, e0, prm.ne);
   __syncthreads();
-  hf_forward<P_, Q_, 2, S1, 0, NEB, NT>(U1, T1, T2, uq1, sBo, sBc);
-  hf_forward<P_, Q_, 2, S1, 1, NEB, NT>(U1, T1, T2, uq1, sBo, sBc);
-  hf_forward<P_, Q_, 2, S1, 2, NEB, NT>(U1, T1, T2, uq1, sBo, sBc);
-  hf_forward<P_, Q_, 2, S2, 0, NEB, NT>(U2, T1, T2, uq2, sBo, sBc);
-  hf_forward<P_, Q_, 2, S2, 1, NEB, NT>(U2, T1, T2, uq2, sBo, sBc);
-  hf_forward<P_, Q_, 2, S2, 2, NEB, NT>(U2, T1, T2, uq2, sBo, sBc);
+  hf_forward<L, S1, 0, NEB, NT>(U1, T1, T2, uq1, sBo, sBc);
+  hf_forward<L, S1, 1, NEB, NT>(U1, T1, T2, uq1, sBo, sBc);
+  hf_forward<L, S1, 2, NEB, NT>(U1, T1, T2, uq1, sBo, sBc);
+  hf_forward<L, S2, 0, NEB, NT>(U2, T1, T2, uq2, sBo, sBc);
+  hf_forward<L, S2, 1, NEB, NT>(U2, T1, T2, uq2, sBo, sBc);
+  hf_forward<L, S2, 2, NEB, NT>(U2, T1, T2, uq2, sBo, sBc);
   // the contribution of every point replaces its first value of space 1
   for (int w = threadIdx.x; w < NEB * Q; w += NT)
   {
@@ -274,32 +290,27 @@ __global__ void __launch_bounds__(NT) flux_hex_error_kernel(HFParams prm)
 
 // ---- production kernels -------------------------------------------------------------------------------------------------
 
+// the cross-check's parameters (tab and CE unread), the scratch of the branch-free scatter and the tables
 template <int P_>
-struct HF7Params
+struct HF7Params : HFParams
 {
-  const int32_t *lidx_a, *lidx_b;  // trial / test (mixed mass), space 1 / space 2 (error integral): [ne][PS]
-  int PS_a, PS_b;
-  const double *qd;     // [ne][10][Q], x-slowest point order
-  const double *ecoef;  // [ne][CE]
-  const double *x_a, *x_b;
-  double *y;            // test-space L-vector (mixed mass) or estimates [ne] (error integral)
-  double *sink;         // scratch of the branch-free scatter
-  int ne;
+  double *sink;
   double Bo[(P_ + 1) * P_];
   double Bc[(P_ + 1) * (P_ + 1)];
 };
 
 // NE elements per batch; per element in shared memory: the q-data [10][Q] and the coefficient block [CE] (TMA destinations), the
 // element dofs U [UE] (one space at a time for the mixed mass, both spaces for the error integral), and per component the work
-// arrays W1 (q, d1, d2), W2 (q, q, d2) sized for the larger of the two spaces, and NV sets of point values V (q, q, q).
-template <int P_, int NE, int NV>
+// arrays W1 (q, d1, d2), W2 (q, q, d2) sized for the larger of the spaces SA, SB, and NV sets of point values V (q, q, q).
+template <int P_, int NE_, int SA, int SB, int NV, int CE_>
 struct HF7Layout
 {
-  static constexpr int q = P_ + 1, n = P_ + 1, Q = q * q * q;
-  static constexpr int PN = HexSpace<P_, SP_ND>::P, PR = HexSpace<P_, SP_RT>::P;
-  static constexpr int UE = NV == 1 ? PN : PN + PR;
-  static constexpr int GE = 10 * Q, CE = NV == 1 ? 10 : 18;  // coefficient blocks: C (+ 1 pad), or C1 | C2
-  static constexpr int W1 = q * n * n, W2 = q * q * n;
+  using Sa = HexSpace<P_, SA>;
+  using Sb = HexSpace<P_, SB>;
+  static constexpr int p = P_, NE = NE_, q = P_ + 1, Q = q * q * q;
+  static constexpr int UE = NV == 1 ? imax(Sa::P, Sb::P) : Sa::P + Sb::P;
+  static constexpr int GE = 10 * Q, CE = CE_;
+  static constexpr int W1 = q * imax(Sa::D12, Sb::D12), W2 = q * q * imax(Sa::D2, Sb::D2);
   static constexpr int OFF_G = 0, OFF_C = OFF_G + NE * GE, OFF_U = OFF_C + NE * CE, OFF_W1 = OFF_U + NE * UE,
                        OFF_W2 = OFF_W1 + 3 * NE * W1, OFF_V = OFF_W2 + 3 * NE * W2, OFF_BAR = (OFF_V + NV * 3 * NE * Q + 1) & ~1;
   static constexpr int SMEM_BYTES = (OFF_BAR + 2) * 8;
@@ -316,15 +327,19 @@ template <> struct HF7Shape<4> { static constexpr int NE = 2, WPC = 2, MINB = 3,
 template <> struct HF7Shape<5> { static constexpr int NE = 2, WPC = 2, MINB = 3, MINB_E = 2; };
 template <> struct HF7Shape<6> { static constexpr int NE = 1, WPC = 2, MINB = 2, MINB_E = 2; };
 
+// The production kernels' rule: q1d = p + 1, p = 2 ... 6 (HF7Shape), and 1-D tables mirror-symmetric within HF7_SYM_TOL of their
+// largest entry.
+constexpr double HF7_SYM_TOL = 8e-15;
+bool hf7_shape(int p, int q1d) { return q1d == p + 1 && p >= 2 && p <= 6; }
+
 // One phase of component C of space S over the batch: every thread of the component's warps owns one line at a time.
 //   PH 0..2: forward along x, y, z (U -> W1 -> W2 -> V);  PH 3..5: transposed along z, y, x (V -> W2 -> W1 -> U)
 // U points at the space's dofs of element 0 (element stride UE), V at the space's point values of element 0.
-template <int P_, int NE, int NV, int S, int C, int PH, int NTC>
-__device__ __forceinline__ void hf7_phase(const HF7Params<P_> &prm, double *sm, double *U, double *V, int t)
+template <typename L, int S, int C, int PH, int NTC>
+__device__ __forceinline__ void hf7_phase(const HF7Params<L::p> &prm, double *sm, double *U, double *V, int t)
 {
-  using L = HF7Layout<P_, NE, NV>;
-  using K = HexComp<P_, S, C>;
-  constexpr int q = L::q, d0 = K::d0, d1 = K::d1, d2 = K::d2, UE = L::UE;
+  using K = HexComp<L::p, S, C>;
+  constexpr int NE = L::NE, q = L::q, d0 = K::d0, d1 = K::d1, d2 = K::d2, UE = L::UE;
   const double *Mx = K::c0 ? prm.Bc : prm.Bo, *My = K::c1 ? prm.Bc : prm.Bo, *Mz = K::c2 ? prm.Bc : prm.Bo;
   double *Uc = U + K::off, *W1 = sm + L::OFF_W1 + C * NE * L::W1, *W2 = sm + L::OFF_W2 + C * NE * L::W2, *Vc = V + C * NE * L::Q;
   constexpr int NP = PH == 0 ? d1 * d2 : PH == 1 || PH == 4 ? q * d2 : PH == 2 || PH == 3 ? q * q : d1 * d2;
@@ -340,24 +355,23 @@ __device__ __forceinline__ void hf7_phase(const HF7Params<P_> &prm, double *sm, 
   }
 }
 
-template <int P_, int NE, int NV, int S, int PH, int NTC>
-__device__ __forceinline__ void hf7_phase_all(const HF7Params<P_> &prm, double *sm, double *U, double *V, int comp, int t)
+template <typename L, int S, int PH, int NTC>
+__device__ __forceinline__ void hf7_phase_all(const HF7Params<L::p> &prm, double *sm, double *U, double *V, int comp, int t)
 {
   if (comp == 0)
-    hf7_phase<P_, NE, NV, S, 0, PH, NTC>(prm, sm, U, V, t);
+    hf7_phase<L, S, 0, PH, NTC>(prm, sm, U, V, t);
   else if (comp == 1)
-    hf7_phase<P_, NE, NV, S, 1, PH, NTC>(prm, sm, U, V, t);
+    hf7_phase<L, S, 1, PH, NTC>(prm, sm, U, V, t);
   else
-    hf7_phase<P_, NE, NV, S, 2, PH, NTC>(prm, sm, U, V, t);
+    hf7_phase<L, S, 2, PH, NTC>(prm, sm, U, V, t);
   __syncthreads();
 }
 
 // Stage the batch's q-data and coefficient blocks behind one mbarrier (thread 0 issues; the caller's next __syncthreads publishes
 // the initialised barrier before anyone polls it).
-template <int P_, int NE, int NV>
-__device__ __forceinline__ void hf7_stage(const HF7Params<P_> &prm, double *sm, uint64_t *bar, int e0, int nel)
+template <typename L>
+__device__ __forceinline__ void hf7_stage(const HF7Params<L::p> &prm, double *sm, uint64_t *bar, int e0, int nel)
 {
-  using L = HF7Layout<P_, NE, NV>;
   mbar_init(bar, 1);
   fence_proxy_async();
   const uint64_t once = l2_evict_first_policy();
@@ -366,24 +380,25 @@ __device__ __forceinline__ void hf7_stage(const HF7Params<P_> &prm, double *sm, 
   tma_bulk_g2s_hint(sm + L::OFF_C, prm.ecoef + (size_t)e0 * L::CE, (uint32_t)(nel * L::CE * sizeof(double)), bar, once);
 }
 
-template <int P_, int NE, int NV, int S, int NT>
+// li: the batch's first restriction row. Row offsets within a batch are 32-bit (e < NE), which keeps them apart from the 64-bit
+// batch offset; a shared 64-bit (e0 + e) PS costs each access a 64-bit multiply.
+template <typename L, int S, int NT>
 __device__ __forceinline__ void hf7_gather(const int32_t *li, int PS, const double *x, double *U, int nel, int tid)
 {
-  using L = HF7Layout<P_, NE, NV>;
-  constexpr int P = HexSpace<P_, S>::P;
-  for (int w = tid; w < NE * P; w += NT)
+  constexpr int P = HexSpace<L::p, S>::P;
+  for (int w = tid; w < L::NE * P; w += NT)
   {
     const int e = w / P, l = w % P;
-    U[e * L::UE + l] = e < nel ? gather1(x, li[(size_t)e * PS + l]) : 0.0;
+    U[e * L::UE + l] = e < nel ? gather1(x, li[e * PS + l]) : 0.0;
   }
 }
 
-// ST: the trial space; the test space is the other one
-template <int P_, int ST, int NE, int WPC, int MINB>
+// ST: the trial space, SS: the test space; CE doubles per coefficient block, C first
+template <int P_, int ST, int SS, int CE, int NE, int WPC, int MINB>
 __global__ void __launch_bounds__(3 * WPC * 32, MINB) flux_hex_mixed7_kernel(const __grid_constant__ HF7Params<P_> prm)
 {
-  using L = HF7Layout<P_, NE, 1>;
-  constexpr int q = L::q, Q = L::Q, SS = 1 - ST, PT = HexSpace<P_, SS>::P, NTC = WPC * 32, NT = 3 * NTC;
+  using L = HF7Layout<P_, NE, ST, SS, 1, CE>;
+  constexpr int q = L::q, Q = L::Q, PT = HexSpace<P_, SS>::P, NTC = WPC * 32, NT = 3 * NTC;
   B2P_DYN_SMEM_ALIGNED16(unsigned char, smem_raw);
   double *sm = (double *)smem_raw;
   double *sG = sm + L::OFF_G, *sC = sm + L::OFF_C, *sU = sm + L::OFF_U, *sV = sm + L::OFF_V;
@@ -392,13 +407,13 @@ __global__ void __launch_bounds__(3 * WPC * 32, MINB) flux_hex_mixed7_kernel(con
   const int e0 = blockIdx.x * NE, nel = min(NE, prm.ne - e0);
   if (nel <= 0) return;
 
-  if (tid == 0) hf7_stage<P_, NE, 1>(prm, sm, bar, e0, nel);
-  hf7_gather<P_, NE, 1, ST, NT>(prm.lidx_a + (size_t)e0 * prm.PS_a, prm.PS_a, prm.x_a, sU, nel, tid);
+  if (tid == 0) hf7_stage<L>(prm, sm, bar, e0, nel);
+  hf7_gather<L, ST, NT>(prm.lidx_a + (size_t)e0 * prm.PS_a, prm.PS_a, prm.x_a, sU, nel, tid);
   __syncthreads();
 
-  hf7_phase_all<P_, NE, 1, ST, 0, NTC>(prm, sm, sU, sV, comp, t);
-  hf7_phase_all<P_, NE, 1, ST, 1, NTC>(prm, sm, sU, sV, comp, t);
-  hf7_phase_all<P_, NE, 1, ST, 2, NTC>(prm, sm, sU, sV, comp, t);
+  hf7_phase_all<L, ST, 0, NTC>(prm, sm, sU, sV, comp, t);
+  hf7_phase_all<L, ST, 1, NTC>(prm, sm, sU, sV, comp, t);
+  hf7_phase_all<L, ST, 2, NTC>(prm, sm, sU, sV, comp, t);
 
   // D: one thread per point, in the x-slowest order of the q-data
   mbar_wait(bar, 0);
@@ -417,25 +432,25 @@ __global__ void __launch_bounds__(3 * WPC * 32, MINB) flux_hex_mixed7_kernel(con
     double *v0 = sV + e * Q + iq, *v1 = v0 + NE * Q, *v2 = v1 + NE * Q;
     const double u[3] = {*v0, *v1, *v2};
     double v[3];
-    mixed_point<ST>(A, C, g[0], u, v);
+    mixed_point<ST, SS>(A, C, g[0], u, v);
     *v0 = v[0];
     *v1 = v[1];
     *v2 = v[2];
   }
   __syncthreads();
 
-  hf7_phase_all<P_, NE, 1, SS, 3, NTC>(prm, sm, sU, sV, comp, t);
-  hf7_phase_all<P_, NE, 1, SS, 4, NTC>(prm, sm, sU, sV, comp, t);
-  hf7_phase_all<P_, NE, 1, SS, 5, NTC>(prm, sm, sU, sV, comp, t);
+  hf7_phase_all<L, SS, 3, NTC>(prm, sm, sU, sV, comp, t);
+  hf7_phase_all<L, SS, 4, NTC>(prm, sm, sU, sV, comp, t);
+  hf7_phase_all<L, SS, 5, NTC>(prm, sm, sU, sV, comp, t);
 
-  // scatter: RED.F64 for every entry; masked entries add 0.0 to this thread's sink slot
+  // scatter: RED.F64 for every entry; masked entries (and the empty slots of a ragged batch) add 0.0 to this thread's sink slot
   const int32_t *li = prm.lidx_b + (size_t)e0 * prm.PS_b;
   double *my_sink = prm.sink + ((blockIdx.x * NT + tid) & (b2p_ctx::SINK_SLOTS - 1));
   for (int w = tid; w < nel * PT; w += NT)
   {
     const int e = w / PT, l = w % PT;
-    const int32_t gi = li[(size_t)e * prm.PS_b + l];
-    const double v = sU[e * L::UE + l];
+    const int32_t gi = li[e * prm.PS_b + l];  // (32-bit row offset, as in hf7_gather)
+    const double v = prm.alpha * sU[e * L::UE + l];
     const bool skip = gi == (int32_t)B2P_SKIP_IDX;
     const int hi = __double2hiint(v) ^ (gi & (int)0x80000000);
     const double sv = skip ? 0.0 : __hiloint2double(hi, __double2loint(v));
@@ -452,8 +467,9 @@ __global__ void __launch_bounds__(3 * WPC * 32, MINB) flux_hex_mixed7_kernel(con
 template <int P_, int S1, int NE, int WPC, int MINB>
 __global__ void __launch_bounds__(3 * WPC * 32, MINB) flux_hex_error7_kernel(const __grid_constant__ HF7Params<P_> prm)
 {
-  using L = HF7Layout<P_, NE, 2>;
-  constexpr int q = L::q, Q = L::Q, S2 = 1 - S1, P1 = HexSpace<P_, S1>::P, NTC = WPC * 32, NT = 3 * NTC;
+  constexpr int S2 = 1 - S1, P1 = HexSpace<P_, S1>::P;
+  using L = HF7Layout<P_, NE, S1, S2, 2, 18>;  // coefficient blocks C1 | C2
+  constexpr int q = L::q, Q = L::Q, NTC = WPC * 32, NT = 3 * NTC;
   B2P_DYN_SMEM_ALIGNED16(unsigned char, smem_raw);
   double *sm = (double *)smem_raw;
   double *sG = sm + L::OFF_G, *sC = sm + L::OFF_C, *sU1 = sm + L::OFF_U, *sU2 = sU1 + P1, *sV1 = sm + L::OFF_V, *sV2 = sV1 + 3 * NE * Q;
@@ -462,17 +478,17 @@ __global__ void __launch_bounds__(3 * WPC * 32, MINB) flux_hex_error7_kernel(con
   const int e0 = blockIdx.x * NE, nel = min(NE, prm.ne - e0);
   if (nel <= 0) return;
 
-  if (tid == 0) hf7_stage<P_, NE, 2>(prm, sm, bar, e0, nel);
-  hf7_gather<P_, NE, 2, S1, NT>(prm.lidx_a + (size_t)e0 * prm.PS_a, prm.PS_a, prm.x_a, sU1, nel, tid);
-  hf7_gather<P_, NE, 2, S2, NT>(prm.lidx_b + (size_t)e0 * prm.PS_b, prm.PS_b, prm.x_b, sU2, nel, tid);
+  if (tid == 0) hf7_stage<L>(prm, sm, bar, e0, nel);
+  hf7_gather<L, S1, NT>(prm.lidx_a + (size_t)e0 * prm.PS_a, prm.PS_a, prm.x_a, sU1, nel, tid);
+  hf7_gather<L, S2, NT>(prm.lidx_b + (size_t)e0 * prm.PS_b, prm.PS_b, prm.x_b, sU2, nel, tid);
   __syncthreads();
 
-  hf7_phase_all<P_, NE, 2, S1, 0, NTC>(prm, sm, sU1, sV1, comp, t);
-  hf7_phase_all<P_, NE, 2, S1, 1, NTC>(prm, sm, sU1, sV1, comp, t);
-  hf7_phase_all<P_, NE, 2, S1, 2, NTC>(prm, sm, sU1, sV1, comp, t);
-  hf7_phase_all<P_, NE, 2, S2, 0, NTC>(prm, sm, sU2, sV2, comp, t);
-  hf7_phase_all<P_, NE, 2, S2, 1, NTC>(prm, sm, sU2, sV2, comp, t);
-  hf7_phase_all<P_, NE, 2, S2, 2, NTC>(prm, sm, sU2, sV2, comp, t);
+  hf7_phase_all<L, S1, 0, NTC>(prm, sm, sU1, sV1, comp, t);
+  hf7_phase_all<L, S1, 1, NTC>(prm, sm, sU1, sV1, comp, t);
+  hf7_phase_all<L, S1, 2, NTC>(prm, sm, sU1, sV1, comp, t);
+  hf7_phase_all<L, S2, 0, NTC>(prm, sm, sU2, sV2, comp, t);
+  hf7_phase_all<L, S2, 1, NTC>(prm, sm, sU2, sV2, comp, t);
+  hf7_phase_all<L, S2, 2, NTC>(prm, sm, sU2, sV2, comp, t);
 
   // the contribution of every point, stored over its first value of space 1 (x-fastest order)
   mbar_wait(bar, 0);
@@ -503,94 +519,146 @@ __global__ void __launch_bounds__(3 * WPC * 32, MINB) flux_hex_error7_kernel(con
   }
 }
 
+// ---- diagonal -----------------------------------------------------------------------------------------------------------
+
+struct RTParams
+{
+  const int32_t *lidx;
+  const double *tab;    // Bo[q][p] | Bc[q][n] | (Gc, unused)
+  const double *qd;     // [ne][10][Q]
+  const double *ecoef;  // [ne][18]: the material tensor (first 9)
+  double *y;
+  int ne;
+  int PS;
+};
+
+// diag[|gid(l)|] += sum_q phi_l(q)^T D_q phi_l(q); one thread per (element, lexicographic dof)
+__global__ void rt_hex_diag_kernel(RTParams prm, int p, int q)
+{
+  const int n = p + 1, D3 = n * p * p, P = 3 * D3, Q = q * q * q;
+  const double *Bo = prm.tab, *Bc = Bo + q * p;
+  const size_t w = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (w >= (size_t)prm.ne * P) return;
+  const int e = (int)(w / P), l = (int)(w % P);
+  const int c = l / D3, r = l % D3;
+  const int d0 = c == 0 ? n : p, d1 = c == 1 ? n : p;
+  const int i = r % d0, j = (r / d0) % d1, k = r / (d0 * d1);
+  double C[9];
+  for (int t = 0; t < 9; t++) C[t] = prm.ecoef[18 * (size_t)e + t];
+  double s = 0.0;
+  for (int qz = 0; qz < q; qz++)
+    for (int qy = 0; qy < q; qy++)
+      for (int qx = 0; qx < q; qx++)
+      {
+        const double fx = c == 0 ? Bc[qx * n + i] : Bo[qx * p + i];
+        const double fy = c == 1 ? Bc[qy * n + j] : Bo[qy * p + j];
+        const double fz = c == 2 ? Bc[qz * n + k] : Bo[qz * p + k];
+        const double f = fx * fy * fz;
+        const double u[3] = {c == 0 ? f : 0.0, c == 1 ? f : 0.0, c == 2 ? f : 0.0};
+        double A[9], Jd[9], v[3];
+        const double *g = prm.qd + (size_t)e * 10 * Q + qslot(q, qx, qy, qz);
+        for (int t = 0; t < 9; t++) A[t] = g[(1 + t) * Q];
+        cofactor33(A, Jd);
+        AtCAx(Jd, C, u, g[0], v);
+        s += u[0] * v[0] + u[1] * v[1] + u[2] * v[2];
+      }
+  int gi = prm.lidx[(size_t)e * prm.PS + l];
+  if (gi == B2P_SKIP_IDX) return;
+  if (gi < 0) gi = -1 - gi;
+  atomicAdd(prm.y + gi, s);
+}
+
 // ---- launchers ----------------------------------------------------------------------------------------------------------
 
-HFParams make_hf_params(const HexFluxArgs &a, const double *xa, const double *xb, double *y, int CE)
+// The kernel parameters of elements [e_off, e_off + e_cnt): restrictions, q-data and coefficient blocks from element e_off on.
+HFParams make_hf_params(const HexFluxArgs &a, int CE, double alpha, const double *xa, const double *xb, double *y, int e_off, int e_cnt)
 {
   HFParams prm;
-  prm.lidx_a = a.lidx_a;
-  prm.lidx_b = a.lidx_b;
+  prm.lidx_a = a.lidx_a + (size_t)e_off * a.PS_a;
+  prm.lidx_b = a.lidx_b + (size_t)e_off * a.PS_b;
   prm.PS_a = a.PS_a;
   prm.PS_b = a.PS_b;
   prm.tab = a.tab;
-  prm.qd = a.geom->qd;
-  prm.ecoef = a.ecoef;
+  prm.qd = a.geom->qd + (size_t)e_off * 10 * a.geom->Q;
+  prm.ecoef = a.ecoef + (size_t)e_off * CE;
   prm.CE = CE;
   prm.x_a = xa;
   prm.x_b = xb;
   prm.y = y;
-  prm.ne = a.geom->ne;
+  prm.alpha = alpha;
+  prm.ne = e_cnt;
   return prm;
 }
 
-template <int P_, int Q_, int NV>
-constexpr int hf_neb()
+// One CTA per batch of `per_batch` elements. A non-null `record` names the kernel in the context's launch record.
+template <typename K, typename Prm>
+int launch_batches(K *kern, const Prm &prm, int threads, size_t shmem, cudaStream_t s, b2p_ctx *ctx, const char *record, int per_batch)
 {
-  constexpr int per_elem_bytes = HFLayout<P_, Q_, NV>::PER_ELEM * 8;
-  return (per_elem_bytes * 8 <= 100 * 1024) ? 8 : (per_elem_bytes * 4 <= 100 * 1024) ? 4 : (per_elem_bytes * 2 <= 200 * 1024) ? 2 : 1;
+  const int grid = (prm.ne + per_batch - 1) / per_batch;
+  if (record) return launch_persistent(kern, prm, threads, shmem, s, false, ctx, record, false, false, grid, 1, per_batch, grid);
+  B2P_LAUNCH(kern, grid, threads, shmem, s, prm);
+  B2P_CUDA(ctx, cudaGetLastError());
+  return B2P_SUCCESS;
 }
 
-template <int P_, int Q_, int SA, bool ERR>
-int launch_hf_pq(const HexFluxArgs &a, const double *xa, const double *xb, double *y, cudaStream_t s)
+template <int P_, int Q_, int SA, int SB, bool ERR>
+int launch_hf_pq(const HexFluxArgs &a, const HFParams &prm, bool record, cudaStream_t s)
 {
-  constexpr int NV = ERR ? 2 : 1, NEB = hf_neb<P_, Q_, NV>(), NT = 256;
-  using L = HFLayout<P_, Q_, NV>;
+  constexpr int NV = ERR ? 2 : 1, NT = 256;
+  using L = HFLayout<P_, Q_, SA, SB, NV>;
+  constexpr int per_elem_bytes = L::PER_ELEM * 8;
+  constexpr int NEB = (per_elem_bytes * 8 <= 100 * 1024) ? 8 : (per_elem_bytes * 4 <= 100 * 1024) ? 4 : (per_elem_bytes * 2 <= 200 * 1024) ? 2 : 1;
   const size_t shmem = (size_t)(Q_ * P_ + Q_ * (P_ + 1) + NEB * L::PER_ELEM) * sizeof(double);
-  auto kern = ERR ? flux_hex_error_kernel<P_, Q_, SA, NEB, NT> : flux_hex_mixed_kernel<P_, Q_, SA, NEB, NT>;
+  auto kern = [] {
+    if constexpr (ERR)
+      return flux_hex_error_kernel<P_, Q_, SA, NEB, NT>;
+    else
+      return flux_hex_mixed_kernel<P_, Q_, SA, SB, NEB, NT>;
+  }();
   if (int rc = configure_kernel(a.ctx, kern, shmem)) return rc;
-  const int grid = (a.geom->ne + NEB - 1) / NEB;  // one CTA per batch
-  return launch_persistent(kern, make_hf_params(a, xa, xb, y, ERR ? 18 : 10), NT, shmem, s, false, a.ctx,
-                           ERR ? "flux_hex_error_kernel" : "flux_hex_mixed_kernel", false, false, grid, 1, NEB, grid);
+  return launch_batches(kern, prm, NT, shmem, s, a.ctx, record ? (ERR ? "flux_hex_error_kernel" : "flux_hex_mixed_kernel") : nullptr, NEB);
 }
 
-template <int P_, int SA, bool ERR>
-int launch_hf7(const HexFluxArgs &a, const double *xa, const double *xb, double *y, cudaStream_t s)
+template <int P_, int SA, int SB, bool ERR, int CE>
+int launch_hf7(const HexFluxArgs &a, const HFParams &base, bool record, cudaStream_t s)
 {
   using S = HF7Shape<P_>;
-  constexpr int NV = ERR ? 2 : 1;
-  using L = HF7Layout<P_, S::NE, NV>;
+  using L = HF7Layout<P_, S::NE, SA, SB, ERR ? 2 : 1, CE>;
   constexpr int NT = 3 * S::WPC * 32;
-  auto kern = ERR ? flux_hex_error7_kernel<P_, SA, S::NE, S::WPC, S::MINB_E> : flux_hex_mixed7_kernel<P_, SA, S::NE, S::WPC, S::MINB>;
+  auto kern = [] {
+    if constexpr (ERR)
+      return flux_hex_error7_kernel<P_, SA, S::NE, S::WPC, S::MINB_E>;
+    else
+      return flux_hex_mixed7_kernel<P_, SA, SB, CE, S::NE, S::WPC, S::MINB>;
+  }();
   if (int rc = configure_kernel(a.ctx, kern, L::SMEM_BYTES)) return rc;
   HF7Params<P_> prm;
-  prm.lidx_a = a.lidx_a;
-  prm.lidx_b = a.lidx_b;
-  prm.PS_a = a.PS_a;
-  prm.PS_b = a.PS_b;
-  prm.qd = a.geom->qd;
-  prm.ecoef = a.ecoef;
-  prm.x_a = xa;
-  prm.x_b = xb;
-  prm.y = y;
+  static_cast<HFParams &>(prm) = base;
   prm.sink = a.ctx->d_sink;
-  prm.ne = a.geom->ne;
   copy_tables(a.h_tab, P_, P_ + 1, P_ + 1, prm.Bo, prm.Bc, nullptr);
-  const int grid = (prm.ne + S::NE - 1) / S::NE;  // one CTA per batch
-  return launch_persistent(kern, prm, NT, L::SMEM_BYTES, s, false, a.ctx, ERR ? "flux_hex_error7_kernel" : "flux_hex_mixed7_kernel", false,
-                           false, grid, 1, S::NE, grid);
+  return launch_batches(kern, prm, NT, L::SMEM_BYTES, s, a.ctx, record ? (ERR ? "flux_hex_error7_kernel" : "flux_hex_mixed7_kernel") : nullptr,
+                        S::NE);
 }
 
-template <bool ERR>
-int launch_hex_flux(const HexFluxArgs &a, const double *xa, const double *xb, double *y, cudaStream_t s)
+// The mixed mass from space SA to space SB with CE-double coefficient blocks, or (ERR) the error integral with SA the space of
+// index 1, on the production kernel (`production`) or the cross-check kernel. `who` and `tag` name the launch in the trace and
+// the error message; `record`: store it in the context's launch record.
+template <int SA, int SB, bool ERR, int CE>
+int launch_hdiv(const HexFluxArgs &a, const HFParams &prm, bool production, bool record, const char *who, const char *tag, cudaStream_t s)
 {
-  if (a.geom->ne <= 0) return B2P_SUCCESS;
+  if (prm.ne <= 0) return B2P_SUCCESS;
   static const bool trace = std::getenv("B2P_TRACE_KERNEL") != nullptr;
   const int p = a.p, q1d = a.geom->q1d;
-  const char *what = ERR ? "error" : "mixed";
-  const char *sp = a.space_a == SP_ND ? (ERR ? "nd,rt" : "nd->rt") : (ERR ? "rt,nd" : "rt->nd");
-  if (a.production)
+  if (trace) fprintf(stderr, "[b2p] %s%s%s p=%d q1d=%d ne=%d\n", who, production ? "7" : "", tag, p, q1d, prm.ne);
+  if (production)
   {
-    if (trace) fprintf(stderr, "[b2p] flux_hex_%s7 %s p=%d q1d=%d ne=%d\n", what, sp, p, q1d, a.geom->ne);
-#define B2P_CASE(PP)                                                                                        \
-  if (p == PP)                                                                                              \
-    return a.space_a == SP_ND ? launch_hf7<PP, SP_ND, ERR>(a, xa, xb, y, s) : launch_hf7<PP, SP_RT, ERR>(a, xa, xb, y, s);
+#define B2P_CASE(PP) \
+  if (p == PP) return launch_hf7<PP, SA, SB, ERR, CE>(a, prm, record, s);
     B2P_CASE(2) B2P_CASE(3) B2P_CASE(4) B2P_CASE(5) B2P_CASE(6)
 #undef B2P_CASE
   }
-  if (trace) fprintf(stderr, "[b2p] flux_hex_%s %s p=%d q1d=%d ne=%d\n", what, sp, p, q1d, a.geom->ne);
-#define B2P_CASE(PP, QQ)                                                                                                   \
-  if (p == PP && q1d == QQ)                                                                                                \
-    return a.space_a == SP_ND ? launch_hf_pq<PP, QQ, SP_ND, ERR>(a, xa, xb, y, s) : launch_hf_pq<PP, QQ, SP_RT, ERR>(a, xa, xb, y, s);
+#define B2P_CASE(PP, QQ) \
+  if (p == PP && q1d == QQ) return launch_hf_pq<PP, QQ, SA, SB, ERR>(a, prm, record, s);
   B2P_CASE(1, 2) B2P_CASE(1, 3) B2P_CASE(1, 4) B2P_CASE(1, 5) B2P_CASE(1, 6) B2P_CASE(1, 7)
   B2P_CASE(2, 3) B2P_CASE(2, 4) B2P_CASE(2, 5) B2P_CASE(2, 6) B2P_CASE(2, 7)
   B2P_CASE(3, 4) B2P_CASE(3, 5) B2P_CASE(3, 6) B2P_CASE(3, 7)
@@ -598,16 +666,25 @@ int launch_hex_flux(const HexFluxArgs &a, const double *xa, const double *xb, do
   B2P_CASE(5, 6) B2P_CASE(5, 7)
   B2P_CASE(6, 7)
 #undef B2P_CASE
-  set_error(a.ctx, "flux_hex_%s: no kernel for p=%d q1d=%d", what, p, q1d);
+  set_error(a.ctx, "%s: no kernel for p=%d q1d=%d", who, p, q1d);
   return B2P_ERR_UNSUPPORTED;
+}
+
+template <bool ERR>
+int launch_hex_flux(const HexFluxArgs &a, const double *xa, const double *xb, double *y, cudaStream_t s)
+{
+  constexpr int CE = ERR ? 18 : 10;  // C1 | C2, or C (+ 1 pad)
+  const HFParams prm = make_hf_params(a, CE, 1.0, xa, xb, y, 0, a.geom->ne);
+  const char *who = ERR ? "flux_hex_error" : "flux_hex_mixed";
+  if (a.space_a == SP_ND) return launch_hdiv<SP_ND, SP_RT, ERR, CE>(a, prm, a.production, true, who, ERR ? " nd,rt" : " nd->rt", s);
+  return launch_hdiv<SP_RT, SP_ND, ERR, CE>(a, prm, a.production, true, who, ERR ? " rt,nd" : " rt->nd", s);
 }
 
 }  // namespace
 
 bool hex_flux_production_eligible(int p, int q1d, const double *h_tab)
 {
-  // the test of rt_hex_apply7_eligible: q1d = p + 1, p = 2 ... 6, tables mirror-symmetric within 8e-15 of the largest entry
-  return q1d == p + 1 && p >= 2 && p <= 6 && nd_tables_symmetric(h_tab, p, q1d, 8e-15);
+  return hf7_shape(p, q1d) && nd_tables_symmetric(h_tab, p, q1d, HF7_SYM_TOL);
 }
 
 int launch_hex_flux_mixed(const HexFluxArgs &a, const double *x, double *y, cudaStream_t s)
@@ -618,6 +695,38 @@ int launch_hex_flux_mixed(const HexFluxArgs &a, const double *x, double *y, cuda
 int launch_hex_flux_error(const HexFluxArgs &a, const double *x1, const double *x2, double *est, cudaStream_t s)
 {
   return launch_hex_flux<true>(a, x1, x2, est, s);
+}
+
+bool rt_hex_apply7_eligible(b2p_op *op)
+{
+  if (!op || op->kind != B2P_RT_MASS || op->dense || !op->ecoef) return false;
+  return hf7_shape(op->p, op->q1d) && nd_tables_symmetric(op, HF7_SYM_TOL);  // (the symmetry cached on the operator)
+}
+
+int launch_rt_hex_apply(b2p_op *op, const int32_t *lidx, double alpha, const double *x, double *y, const ApplyRange &rg, cudaStream_t s,
+                        bool rt7)
+{
+  HexFluxArgs a;
+  a.ctx = op->ctx;
+  a.geom = op->geom;
+  a.p = op->p;
+  a.h_tab = op->h_tab.data();
+  a.tab = op->tab;
+  a.lidx_a = a.lidx_b = lidx;
+  a.PS_a = a.PS_b = op->PS;
+  a.ecoef = op->ecoef;
+  const HFParams prm = make_hf_params(a, 18, alpha, x, nullptr, y, rg.e_off, range_count(op, rg));
+  return launch_hdiv<SP_RT, SP_RT, false, 18>(a, prm, rt7, false, "rt_hex_apply", "", s);
+}
+
+int launch_rt_hex_diag(b2p_op *op, double *diag, cudaStream_t s)
+{
+  const size_t total = (size_t)op->ne * op->P;
+  const int nt = 128;
+  const RTParams prm = {op->lidx, op->tab, op->geom->qd, op->ecoef, diag, op->ne, op->PS};
+  B2P_LAUNCH(rt_hex_diag_kernel, (unsigned)((total + nt - 1) / nt), nt, 0, s, prm, op->p, op->q1d);
+  B2P_CUDA(op->ctx, cudaGetLastError());
+  return B2P_SUCCESS;
 }
 
 }  // namespace b2p

@@ -342,7 +342,8 @@ bool op_essential_matches(const b2p_op *op, const int32_t *ess_ldofs, int64_t n)
 int apply_range(b2p_op *op, const int32_t *lidx, double alpha, const double *x, double *y, const ApplyRange &rg, int flags,
                 cudaStream_t s);
 int launch_nd_hex_diag(b2p_op *op, double *diag, cudaStream_t s);
-// Raviart-Thomas mass (b2p_hex_rt.cu): rt_hex_apply7_kernel with `rt7`, the cross-check kernel otherwise
+// Raviart-Thomas mass (b2p_hex_flux.cu, the mixed mass with RT as trial and test space): flux_hex_mixed7_kernel with `rt7`, the
+// cross-check kernel otherwise
 bool rt_hex_apply7_eligible(b2p_op *op);
 int launch_rt_hex_apply(b2p_op *op, const int32_t *lidx, double alpha, const double *x, double *y, const ApplyRange &rg, cudaStream_t s,
                         bool rt7);
@@ -351,8 +352,9 @@ int launch_rt_hex_diag(b2p_op *op, double *diag, cudaStream_t s);
 // restriction builder: b2p_op_create, b2p_op_coarsen and b2p_flux_estimator_create_hex); rows padded to *PS = P rounded up to 4
 // with B2P_SKIP_IDX. `who` prefixes the error messages.
 int build_lex_restriction(b2p_ctx *ctx, const char *who, const b2p_op_desc *d, int P, int64_t lsize, int ne, int *PS, int32_t **lidx);
-// Flux operator and error integrals of the flux estimator on hexahedra (b2p_hex_flux.cu). Space a is the trial space of the mixed
-// mass (the test space is b) or the space of index 1 of the error integral (index 2 is b); space_a: 0 = Nedelec, 1 = Raviart-Thomas.
+// Flux operator and error integrals of the flux estimator on hexahedra (b2p_hex_flux.cu, which also fills these for the
+// Raviart-Thomas mass). Space a is the trial space of the mixed mass (the test space is b) or the space of index 1 of the error
+// integral (index 2 is b); space_a: 0 = Nedelec, 1 = Raviart-Thomas.
 struct HexFluxArgs
 {
   b2p_ctx *ctx = nullptr;
@@ -364,7 +366,7 @@ struct HexFluxArgs
   int space_a = 0;
   const int32_t *lidx_a = nullptr, *lidx_b = nullptr;
   int PS_a = 0, PS_b = 0;
-  const double *ecoef = nullptr;  // [ne][10] {C, pad} (mixed mass) or [ne][18] {C1, C2} (error integral)
+  const double *ecoef = nullptr;  // [ne][10] {C, pad} (Flux), [ne][18] {C1, C2} (error integral) or b2p_op::ecoef (RT mass)
 };
 bool hex_flux_production_eligible(int p, int q1d, const double *h_tab);
 // y_b += Flux x_a

@@ -1,4 +1,4 @@
-"""GPU: the sum-factorised Raviart-Thomas mass on hexahedra (kind B2P_RT_MASS, b2p_hex_rt.cu) against the oracle's H(div) mass matrix
+"""GPU: the sum-factorised Raviart-Thomas mass on hexahedra (kind B2P_RT_MASS, b2p_hex_flux.cu) against the oracle's H(div) mass matrix
 and the dense-table operator, its diagonal, masked restriction, assembled RT_0 matrix, p-coarsening, refusals, and the grad-flux
 estimator of the cylinder cavity with the sum-factorised RT mass under Jacobi and under the RT / ND p-multigrid. Bound: the operator
 bound ||dy|| <= 1e-12 ||y|| unless stated otherwise."""

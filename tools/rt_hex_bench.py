@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Raviart-Thomas mass on hexahedra: the dense-table operator (b2p_operator_vecfe_mass) against the sum-factorised one (B2P_RT_MASS,
-rt_hex_apply7_kernel), alternated in one process at about 2M RT dofs, and the grad-flux projection of one cylinder-cavity mode with
-Jacobi PCG against multigrid PCG.
+flux_hex_mixed7_kernel with RT as trial and test space), alternated in one process at about 2M RT dofs, and the grad-flux projection
+of one cylinder-cavity mode with Jacobi PCG against multigrid PCG.
 
   apply       p = 2 ... 6 at q1d = p + 1 on an n^3 box: ms per Mult (CUDA events around each Mult, L2 flushed before it, median over
               the rounds of the per-round means), algorithmic bytes per Mult (x and y per unique dof, a 4-byte index per element dof,
