@@ -270,6 +270,29 @@ typedef struct
   const double *mat;              /* [out_P][in_P] */
 } b2p_dense_interp_desc;
 int b2p_interp_create_dense(b2p_ctx *ctx, const b2p_dense_interp_desc *desc, b2p_interp **out);
+/* Discrete curl C : ND_p -> RT_{p-1} on hexahedra (SpaceOperator::GetCurlMatrix, a DiscreteLinearOperator with a
+ * CurlInterpolator, fem/fespace.cpp:204,216), sum-factorised: per element, in lexicographic order, RT component c equals
+ * D_a u_b - D_b u_a for (c, a, b) cyclic, with D acting along one axis and the identity along the other two; no element
+ * matrix is formed. ND component b is open (p Gauss-Legendre nodes) along axis b and closed (p + 1 Gauss-Lobatto nodes) along
+ * the others; RT component c is closed along c and open along the others. The ND space is described as in b2p_op_desc of
+ * B2P_ND_MASS (native idx + orient + GetDofMap()), the RT space as in B2P_RT_MASS (lexicographic idx + signs, dof_map NULL).
+ * The result is an ordinary b2p_interp with the Mult / MultTranspose multiplicity scaling of b2p_interp_create (1/mult of
+ * the RT space), one kernel launch per apply. B2P_ERR_ARG: a null pointer, ne < 1, p < 1, an lsize outside 1..2^31-1, an index
+ * outside [0, lsize) or a dof_map entry outside the element; B2P_ERR_UNSUPPORTED: p > 6. */
+typedef struct
+{
+  int ne, p;              /* ND_p -> RT_{p-1}; p as in b2p_op_desc of B2P_ND_MASS / B2P_RT_MASS */
+  int64_t nd_lsize;
+  const int32_t *nd_idx;  /* [ne][3 p (p+1)^2] native order */
+  const int8_t *nd_orient;
+  const int32_t *nd_dof_map;
+  int64_t rt_lsize;
+  const int32_t *rt_idx;  /* [ne][3 p^2 (p+1)] */
+  const int8_t *rt_orient;
+  const int32_t *rt_dof_map; /* may be NULL */
+  const double *D;        /* [p][p+1] row-major: closed-basis derivative at the open nodes (ProjectCurl) */
+} b2p_curl_interp_desc;
+int b2p_interp_create_curl_hex(b2p_ctx *ctx, const b2p_curl_interp_desc *desc, b2p_interp **out);
 int b2p_interp_apply_add(b2p_interp *it, int transpose, double alpha, const double *x, double *y, b2p_stream s);
 void b2p_interp_destroy(b2p_interp *it);
 

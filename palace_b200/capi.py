@@ -325,8 +325,16 @@ class DenseInterpDesc(C.Structure):
     ]
 
 
+class CurlInterpDesc(C.Structure):
+    _fields_ = [
+        ("ne", C.c_int), ("p", C.c_int), ("nd_lsize", C.c_int64), ("nd_idx", C.c_void_p), ("nd_orient", C.c_void_p),
+        ("nd_dof_map", C.c_void_p), ("rt_lsize", C.c_int64), ("rt_idx", C.c_void_p), ("rt_orient", C.c_void_p),
+        ("rt_dof_map", C.c_void_p), ("D", C.c_void_p),
+    ]
+
+
 class Interp:
-    """Element-local tensor interpolator between two hex spaces (p-prolongation, discrete gradient)."""
+    """Element-local tensor interpolator between two hex spaces (p-prolongation, discrete gradient, discrete curl)."""
 
     def __init__(self, ctx, in_space, out_space, comps):
         """in_space/out_space: dicts(P, lsize, idx, orient, dof_map); comps: list of
@@ -385,6 +393,39 @@ class Interp:
         self = cls.__new__(cls)
         self.ctx, self.h = ctx, h
         self.in_lsize, self.out_lsize = int(in_lsize), int(out_lsize)
+        return self
+
+    @classmethod
+    def curl_hex(cls, ctx, nd_space, rt_space, p):
+        """Discrete curl ND_p -> RT_{p-1} on hexahedra (sum-factorised, b2p_interp_create_curl_hex): Mult gives B = curl E on the
+        RT dofs. nd_space / rt_space: dicts of host.assemble.space_dict."""
+        from .host import assemble as asm
+
+        p = int(p)
+        d = CurlInterpDesc()
+        keep = []
+        ne = np.shape(nd_space["idx"])[0]
+        for pre, sp, P in (("nd", nd_space, 3 * p * (p + 1) ** 2), ("rt", rt_space, 3 * p * p * (p + 1))):
+            idx = _np(sp["idx"], np.int32)
+            if idx.shape != (ne, P):
+                raise ValueError(f"curl_hex: {pre} idx has shape {idx.shape}, expected ({ne}, {P}) for p={p}")
+            keep.append(idx)
+            setattr(d, pre + "_lsize", int(sp["lsize"]))
+            setattr(d, pre + "_idx", _ptr(idx))
+            for key, dtype, shape in (("orient", np.int8, (ne, P)), ("dof_map", np.int32, (P,))):
+                if sp.get(key) is not None:
+                    a = _np(sp[key], dtype)
+                    if a.shape != shape:
+                        raise ValueError(f"curl_hex: {pre} {key} has shape {a.shape}, expected {shape}")
+                    keep.append(a)
+                    setattr(d, f"{pre}_{key}", _ptr(a))
+        D = _np(asm.curl_table(p), np.float64)
+        d.ne, d.p, d.D = ne, p, _ptr(D)
+        h = C.c_void_p()
+        _chk(lib().b2p_interp_create_curl_hex(ctx.h, C.byref(d), C.byref(h)), ctx.h)
+        self = cls.__new__(cls)
+        self.ctx, self.h = ctx, h
+        self.in_lsize, self.out_lsize = int(nd_space["lsize"]), int(rt_space["lsize"])
         return self
 
     def apply_add(self, x, y, transpose=False, alpha=1.0, stream=None):

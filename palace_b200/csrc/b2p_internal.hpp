@@ -187,6 +187,9 @@ struct b2p_interp
   bool dense = false;
   double *dmat = nullptr;
   int8_t *in_co = nullptr, *out_co = nullptr;  // [ne][P][3] rows or null
+  // hexahedral discrete curl ND_p -> RT_{p-1} (b2p_interp_create_curl_hex) when curl_p > 0: in = ND, out = RT, both lexicographic
+  int curl_p = 0;
+  double *curl_D = nullptr;  // [p][p+1] closed-basis derivative at the open nodes
 };
 
 namespace b2p

@@ -6,7 +6,9 @@
 // identity QFunction (/root/reference/palace/fem/libceed/integrator.cpp:515-548); the output is scaled
 // by the inverse dof multiplicity on Mult and the input on MultTranspose
 // (/root/reference/palace/fem/libceed/operator.cpp:182-212). On hexes that dense matrix is a Kronecker
-// product of 1-D matrices per vector component; it is applied here in that factored form.
+// product of 1-D matrices per vector component; it is applied here in that factored form. The discrete curl ND_p -> RT_{p-1}
+// (CurlInterpolator, fespace.cpp:204,216) is a sum of two such products per output component, each reading a different
+// input block; it has a kernel of its own (curl_hex_kernel) that applies both in one pass.
 #include <algorithm>
 #include <cstdlib>
 
@@ -267,6 +269,171 @@ __global__ void __launch_bounds__(256) dense_interp_kernel(DenseInterpParams prm
   }
 }
 
+// Discrete curl C : ND_p -> RT_{p-1} on hexahedra (mfem ProjectCurl, hexspace.discrete_curl_matrix), lexicographic on both
+// sides. ND component b is open (p Gauss-Legendre nodes) along axis b and closed (p + 1 Gauss-Lobatto nodes) along the other
+// two; RT component c is closed along c and open along the other two. For (c, a, b) cyclic, RT_c = D_a u_b - D_b u_a, where
+// D [p][p+1] is the derivative of the closed 1-D basis at the open nodes acting along one axis, the identity along the rest:
+// 2 (p + 1) FMAs per RT dof on Mult, 2 p per ND dof on MultTranspose, no element matrix.
+template <int P>
+struct CurlHex
+{
+  static constexpr int N = P + 1;
+  static constexpr int ND_BLK = P * N * N, RT_BLK = N * P * P;
+  static constexpr int ND_P = 3 * ND_BLK, RT_P = 3 * RT_BLK;
+  // extent of ND block b / RT block c along axis d, and its stride (x fastest)
+  static constexpr int nd_n(int b, int d) { return d == b ? P : N; }
+  static constexpr int rt_n(int c, int d) { return d == c ? N : P; }
+  static constexpr int nd_stride(int b, int d) { return d == 0 ? 1 : d == 1 ? nd_n(b, 0) : nd_n(b, 0) * nd_n(b, 1); }
+  static constexpr int rt_stride(int c, int d) { return d == 0 ? 1 : d == 1 ? rt_n(c, 0) : rt_n(c, 0) * rt_n(c, 1); }
+};
+constexpr int CURL_HEX_PMAX = 6;
+constexpr int CURL_HEX_NT = 256;
+// elements per block: at least two destination dofs per thread
+constexpr int curl_hex_neb(int dst_P) { return (2 * CURL_HEX_NT + dst_P - 1) / dst_P; }
+
+// RT component C at offset r inside its block, from the ND element vector u
+template <int P, int C>
+__device__ __forceinline__ double curl_rt_comp(const double *u, const double *D, int r)
+{
+  using H = CurlHex<P>;
+  constexpr int A = (C + 1) % 3, B = (C + 2) % 3;
+  constexpr int n0 = H::rt_n(C, 0), n1 = H::rt_n(C, 1);
+  const int ix[3] = {r % n0, (r / n0) % n1, r / (n0 * n1)};
+  // D_a u_b runs over u_b's closed index along a; D_b u_a over u_a's closed index along b
+  int jb[3] = {ix[0], ix[1], ix[2]}, ja[3] = {ix[0], ix[1], ix[2]};
+  jb[A] = 0;
+  ja[B] = 0;
+  const double *ub = u + B * H::ND_BLK + jb[0] * H::nd_stride(B, 0) + jb[1] * H::nd_stride(B, 1) + jb[2] * H::nd_stride(B, 2);
+  const double *ua = u + A * H::ND_BLK + ja[0] * H::nd_stride(A, 0) + ja[1] * H::nd_stride(A, 1) + ja[2] * H::nd_stride(A, 2);
+  const double *Da = D + ix[A] * H::N, *Db = D + ix[B] * H::N;
+  double s = 0.0;
+#pragma unroll
+  for (int t = 0; t < H::N; t++) s += Da[t] * ub[t * H::nd_stride(B, A)] - Db[t] * ua[t * H::nd_stride(A, B)];
+  return s;
+}
+
+// ND component B at offset r inside its block, from the RT element vector v (transpose): u_B feeds RT_{A2} through D_{A1}
+// with sign -1 and RT_{A1} through D_{A2} with sign +1, for A1 = B + 1 and A2 = B + 2 (mod 3)
+template <int P, int B>
+__device__ __forceinline__ double curl_nd_comp(const double *v, const double *D, int r)
+{
+  using H = CurlHex<P>;
+  constexpr int A1 = (B + 1) % 3, A2 = (B + 2) % 3;
+  constexpr int n0 = H::nd_n(B, 0), n1 = H::nd_n(B, 1);
+  const int ix[3] = {r % n0, (r / n0) % n1, r / (n0 * n1)};
+  int jp[3] = {ix[0], ix[1], ix[2]}, jm[3] = {ix[0], ix[1], ix[2]};
+  jp[A2] = 0;
+  jm[A1] = 0;
+  const double *vp = v + A1 * H::RT_BLK + jp[0] * H::rt_stride(A1, 0) + jp[1] * H::rt_stride(A1, 1) + jp[2] * H::rt_stride(A1, 2);
+  const double *vm = v + A2 * H::RT_BLK + jm[0] * H::rt_stride(A2, 0) + jm[1] * H::rt_stride(A2, 1) + jm[2] * H::rt_stride(A2, 2);
+  const double *Dp = D + ix[A2], *Dm = D + ix[A1];  // column of D, stride N
+  double s = 0.0;
+#pragma unroll
+  for (int t = 0; t < P; t++) s += Dp[t * H::N] * vp[t * H::rt_stride(A1, A2)] - Dm[t * H::N] * vm[t * H::rt_stride(A2, A1)];
+  return s;
+}
+
+struct CurlParams
+{
+  const int32_t *nd_lidx, *rt_lidx;  // signed lexicographic restrictions [ne][PS]
+  const double *inv_mult, *D, *x;    // inv_mult: of the RT space
+  double *y;
+  double alpha;
+  int ne, nd_PS, rt_PS;
+};
+
+// Mult:           y_rt += alpha (1/mult_rt) sum_e E_rt^T C E_nd x
+// MultTranspose:  y_nd += alpha sum_e E_nd^T C^T E_rt ((1/mult_rt) x)
+template <int P, bool TRANSPOSE>
+__global__ void __launch_bounds__(CURL_HEX_NT) curl_hex_kernel(CurlParams prm)
+{
+  using H = CurlHex<P>;
+  constexpr int SRC = TRANSPOSE ? H::RT_P : H::ND_P, DST = TRANSPOSE ? H::ND_P : H::RT_P;
+  constexpr int NEB = curl_hex_neb(DST);
+  __shared__ double sD[P * H::N];
+  __shared__ double sv[NEB * SRC];
+  const int32_t *src_lidx = TRANSPOSE ? prm.rt_lidx : prm.nd_lidx, *dst_lidx = TRANSPOSE ? prm.nd_lidx : prm.rt_lidx;
+  const int src_PS = TRANSPOSE ? prm.rt_PS : prm.nd_PS, dst_PS = TRANSPOSE ? prm.nd_PS : prm.rt_PS;
+  for (int i = threadIdx.x; i < P * H::N; i += CURL_HEX_NT) sD[i] = prm.D[i];
+  const int e0 = blockIdx.x * NEB;
+#pragma unroll
+  for (int k = 0; k < (NEB * SRC + CURL_HEX_NT - 1) / CURL_HEX_NT; k++)
+  {
+    const int w = threadIdx.x + k * CURL_HEX_NT;
+    if (w >= NEB * SRC) break;
+    const int e = w / SRC, l = w - e * SRC;
+    double v = 0.0;
+    if (e0 + e < prm.ne)
+    {
+      const int32_t gi = src_lidx[(size_t)(e0 + e) * src_PS + l];
+      v = gather1(prm.x, gi);
+      if (TRANSPOSE && gi != B2P_SKIP_IDX) v *= prm.inv_mult[gi >= 0 ? gi : -1 - gi];
+    }
+    sv[w] = v;
+  }
+  __syncthreads();
+  for (int w = threadIdx.x; w < NEB * DST; w += CURL_HEX_NT)
+  {
+    const int e = w / DST, l = w - e * DST;
+    if (e0 + e >= prm.ne) break;
+    const double *src = sv + e * SRC;
+    constexpr int BLK = TRANSPOSE ? H::ND_BLK : H::RT_BLK;
+    const int c = l / BLK, r = l - c * BLK;
+    double s;
+    if (!TRANSPOSE)
+      s = c == 0 ? curl_rt_comp<P, 0>(src, sD, r) : c == 1 ? curl_rt_comp<P, 1>(src, sD, r) : curl_rt_comp<P, 2>(src, sD, r);
+    else
+      s = c == 0 ? curl_nd_comp<P, 0>(src, sD, r) : c == 1 ? curl_nd_comp<P, 1>(src, sD, r) : curl_nd_comp<P, 2>(src, sD, r);
+    const int32_t gi = dst_lidx[(size_t)(e0 + e) * dst_PS + l];
+    if (!TRANSPOSE && gi != B2P_SKIP_IDX) s *= prm.inv_mult[gi >= 0 ? gi : -1 - gi];
+    scatter1(prm.y, gi, prm.alpha * s);
+  }
+}
+
+template <int P, bool TRANSPOSE>
+void curl_hex_launch(const CurlParams &prm, cudaStream_t s)
+{
+  constexpr int NEB = curl_hex_neb(TRANSPOSE ? CurlHex<P>::ND_P : CurlHex<P>::RT_P);
+  void (*kern)(CurlParams) = curl_hex_kernel<P, TRANSPOSE>;
+  B2P_LAUNCH(kern, (prm.ne + NEB - 1) / NEB, CURL_HEX_NT, 0, s, prm);
+}
+
+template <int P>
+void curl_hex_launch(bool transpose, const CurlParams &prm, cudaStream_t s)
+{
+  if (transpose)
+    curl_hex_launch<P, true>(prm, s);
+  else
+    curl_hex_launch<P, false>(prm, s);
+}
+
+int curl_hex_apply(const b2p_interp *it, bool transpose, double alpha, const double *x, double *y, cudaStream_t s)
+{
+  CurlParams prm;
+  prm.nd_lidx = it->in_lidx;
+  prm.rt_lidx = it->out_lidx;
+  prm.inv_mult = it->inv_mult;
+  prm.D = it->curl_D;
+  prm.x = x;
+  prm.y = y;
+  prm.alpha = alpha;
+  prm.ne = it->ne;
+  prm.nd_PS = it->in_PS;
+  prm.rt_PS = it->out_PS;
+  switch (it->curl_p)
+  {
+    case 1: curl_hex_launch<1>(transpose, prm, s); break;
+    case 2: curl_hex_launch<2>(transpose, prm, s); break;
+    case 3: curl_hex_launch<3>(transpose, prm, s); break;
+    case 4: curl_hex_launch<4>(transpose, prm, s); break;
+    case 5: curl_hex_launch<5>(transpose, prm, s); break;
+    case 6: curl_hex_launch<6>(transpose, prm, s); break;
+    default: B2P_CHECK(it->ctx, false, B2P_ERR_UNSUPPORTED, "curl interpolator: p=%d", it->curl_p);
+  }
+  B2P_CUDA(it->ctx, cudaGetLastError());
+  return B2P_SUCCESS;
+}
+
 InterpParams make_params(const b2p_interp *it, double alpha, const double *x, double *y)
 {
   InterpParams p;
@@ -327,10 +494,24 @@ int build_lidx(b2p_ctx *ctx, int ne, int P, int64_t lsize, const int32_t *idx, c
   return upload(ctx, lidx.data(), lidx.size(), d_out);
 }
 
+// 1 / (local elements touching the dof) of the output space, from its signed restriction
+int upload_inv_mult(b2p_ctx *ctx, const std::vector<int32_t> &out_lidx, int64_t out_lsize, double **d_out)
+{
+  std::vector<double> mult((size_t)out_lsize, 0.0);
+  for (int32_t g : out_lidx)
+  {
+    if (g == (int32_t)B2P_SKIP_IDX) continue;
+    mult[g >= 0 ? g : -1 - g] += 1.0;
+  }
+  for (auto &m : mult) m = m > 0.0 ? 1.0 / m : 0.0;
+  return upload(ctx, mult.data(), mult.size(), d_out);
+}
+
 }  // namespace
 
 int interp_apply(const b2p_interp *it, bool transpose, double alpha, const double *x, double *y, cudaStream_t s)
 {
+  if (it->curl_p) return curl_hex_apply(it, transpose, alpha, x, y, s);
   if (it->dense)
   {
     DenseInterpParams dp;
@@ -404,14 +585,7 @@ int b2p_interp_create(b2p_ctx *ctx, const b2p_interp_desc *d, b2p_interp **out)
   if ((rc = build_lidx(ctx, d->ne, d->out_P, d->out_lsize, d->out_idx, d->out_orient, d->out_dof_map, &it->out_PS, &it->out_lidx,
                        &out_host)))
     return rc;
-  std::vector<double> mult((size_t)d->out_lsize, 0.0);
-  for (int32_t g : out_host)
-  {
-    if (g == (int32_t)B2P_SKIP_IDX) continue;
-    mult[g >= 0 ? g : -1 - g] += 1.0;
-  }
-  for (auto &m : mult) m = m > 0.0 ? 1.0 / m : 0.0;
-  if ((rc = upload(ctx, mult.data(), mult.size(), &it->inv_mult))) return rc;
+  if ((rc = upload_inv_mult(ctx, out_host, d->out_lsize, &it->inv_mult))) return rc;
   // B2P_INTERP_OWNER=1 (opt-in until measured): Mult computes every output dof in its first element only (the
   // interpolators of a conforming hierarchy give the same value from every element; the reference averages them,
   // operator.cpp:186-189) -- ~44 % fewer outputs to form, no atomics, no multiplicity gather.
@@ -484,17 +658,44 @@ int b2p_interp_create_dense(b2p_ctx *ctx, const b2p_dense_interp_desc *d, b2p_in
     b2p_interp_destroy(it);
     return rc;
   }
-  std::vector<double> mult((size_t)d->out_lsize, 0.0);
-  for (int32_t g : out_host)
-  {
-    if (g == (int32_t)B2P_SKIP_IDX) continue;
-    mult[g >= 0 ? g : -1 - g] += 1.0;
-  }
-  for (auto &m : mult) m = m > 0.0 ? 1.0 / m : 0.0;
-  if ((rc = upload(ctx, mult.data(), mult.size(), &it->inv_mult)) ||
+  if ((rc = upload_inv_mult(ctx, out_host, d->out_lsize, &it->inv_mult)) ||
       (rc = upload(ctx, d->mat, (size_t)d->out_P * d->in_P, &it->dmat)) ||
       (d->in_curl_orient && (rc = upload(ctx, d->in_curl_orient, (size_t)d->ne * d->in_P * 3, &it->in_co))) ||
       (d->out_curl_orient && (rc = upload(ctx, d->out_curl_orient, (size_t)d->ne * d->out_P * 3, &it->out_co))))
+  {
+    b2p_interp_destroy(it);
+    return rc;
+  }
+  *out = it;
+  return B2P_SUCCESS;
+}
+
+int b2p_interp_create_curl_hex(b2p_ctx *ctx, const b2p_curl_interp_desc *d, b2p_interp **out)
+{
+  B2P_CHECK(ctx, ctx && d && out && d->nd_idx && d->rt_idx && d->D, B2P_ERR_ARG, "b2p_interp_create_curl_hex: null argument");
+  B2P_CHECK(ctx, d->ne > 0, B2P_ERR_ARG, "b2p_interp_create_curl_hex: ne=%d, no elements", d->ne);
+  B2P_CHECK(ctx, d->p >= 1, B2P_ERR_ARG, "b2p_interp_create_curl_hex: p=%d, must be at least 1", d->p);
+  B2P_CHECK(ctx, d->p <= CURL_HEX_PMAX, B2P_ERR_UNSUPPORTED, "b2p_interp_create_curl_hex: p=%d, kernels exist for p = 1..%d", d->p,
+            CURL_HEX_PMAX);
+  B2P_CHECK(ctx, d->nd_lsize > 0 && d->nd_lsize <= INT32_MAX && d->rt_lsize > 0 && d->rt_lsize <= INT32_MAX, B2P_ERR_ARG,
+            "b2p_interp_create_curl_hex: nd_lsize=%lld / rt_lsize=%lld outside 1..2^31-1", (long long)d->nd_lsize,
+            (long long)d->rt_lsize);
+  const int p = d->p, n = p + 1;
+  b2p_interp *it = new b2p_interp;
+  it->ctx = ctx;
+  it->curl_p = p;
+  it->ne = d->ne;
+  it->in_P = 3 * p * n * n;
+  it->out_P = 3 * n * p * p;
+  it->in_lsize = d->nd_lsize;
+  it->out_lsize = d->rt_lsize;
+  it->ncomp = 0;
+  int rc;
+  std::vector<int32_t> out_host;
+  if ((rc = build_lidx(ctx, d->ne, it->in_P, d->nd_lsize, d->nd_idx, d->nd_orient, d->nd_dof_map, &it->in_PS, &it->in_lidx, nullptr)) ||
+      (rc = build_lidx(ctx, d->ne, it->out_P, d->rt_lsize, d->rt_idx, d->rt_orient, d->rt_dof_map, &it->out_PS, &it->out_lidx,
+                       &out_host)) ||
+      (rc = upload_inv_mult(ctx, out_host, d->rt_lsize, &it->inv_mult)) || (rc = upload(ctx, d->D, (size_t)p * n, &it->curl_D)))
   {
     b2p_interp_destroy(it);
     return rc;
@@ -520,6 +721,7 @@ void b2p_interp_destroy(b2p_interp *it)
   cudaFree(it->dmat);
   cudaFree(it->in_co);
   cudaFree(it->out_co);
+  cudaFree(it->curl_D);
   delete it;
 }
 

@@ -77,12 +77,18 @@ def h1_prolongation_comps(pc, pf):
     return [dict(in_off=0, in_n=[pc + 1] * 3, out_off=0, out_n=[pf + 1] * 3, A=[Cc, Cc, Cc])]
 
 
+def curl_table(p):
+    """D [p][p+1]: derivative of the closed (Gauss-Lobatto) 1-D basis at the open (Gauss-Legendre) nodes, the 1-D factor of the
+    discrete gradient (ProjectGrad) and of the discrete curl (ProjectCurl) on hexahedra."""
+    op, _ = hs.gauss_legendre(p)
+    cp = hs.gauss_lobatto(p + 1)
+    return hs.lagrange_table(cp, op)[1]
+
+
 def gradient_comps(p):
     """Kronecker factors of the discrete gradient H1(p) -> ND(p) (ProjectGrad): derivative of the
     closed basis at the open points along the component's axis, identity along the others."""
-    op, _ = hs.gauss_legendre(p)
-    cp = hs.gauss_lobatto(p + 1)
-    _, dC = hs.lagrange_table(cp, op)  # [p, p+1]
+    dC = curl_table(p)  # [p, p+1]
     n = p + 1
     I = np.eye(n)
     d3 = p * n * n
@@ -94,3 +100,27 @@ def gradient_comps(p):
         A[c] = dC
         comps.append(dict(in_off=0, in_n=[n] * 3, out_off=c * d3, out_n=out_n, A=A))
     return comps
+
+
+def curl_kron_terms(p):
+    """The discrete curl ND(p) -> RT(p-1) as two sums of Kronecker factors, one per term of RT_c = D_a u_b - D_b u_a ((c, a, b)
+    cyclic): the form two b2p_interp_create handles applied one after the other take. Interp.curl_hex applies both terms in one
+    pass; this form is its cross-check."""
+    D = curl_table(p)
+    n = p + 1
+    Ip, In = np.eye(p), np.eye(n)
+    d3_nd, d3_rt = p * n * n, n * p * p
+    terms = [[], []]
+    for c in range(3):
+        a, b = (c + 1) % 3, (c + 2) % 3
+        out_n = [p] * 3
+        out_n[c] = n
+        for t, (src, ax, sign) in enumerate(((b, a, 1.0), (a, b, -1.0))):  # + D_a u_b, - D_b u_a
+            in_n = [n] * 3
+            in_n[src] = p
+            A = [None] * 3
+            A[ax] = sign * D
+            A[src] = Ip
+            A[c] = In
+            terms[t].append(dict(in_off=src * d3_nd, in_n=in_n, out_off=c * d3_rt, out_n=out_n, A=A))
+    return terms
